@@ -937,16 +937,17 @@ int lpcnet_b200_debug_frame_network(LPCNetB200Batch *b, const float *features, i
 
 // Test hook (host only, no CUDA): the shared-memory image and its run-time layout words
 // layout[8] = {wA, metaA, wB, metaB, image_bytes, total_bytes, nblkA_padded, nblkB_padded}; also returns sm_image in layout[8].
+// layout[21] = 1 when the model's accumulator bound allows the conversion-free rounding (DeviceModel::fast_cvt).
 int lpcnet_b200_debug_image(const unsigned char *blob, int len, unsigned char *out, size_t cap, uint32_t *layout)
 {
-    SmemLayout L; Geom G;
-    int r = debug_build_image(blob, len, out, cap, &L, &G);
+    SmemLayout L; Geom G; int fast_cvt = 0;
+    int r = debug_build_image(blob, len, out, cap, &L, &G, &fast_cvt);
     if (r < 0) return r;
     layout[0] = L.wA; layout[1] = L.metaA; layout[2] = L.wB; layout[3] = L.metaB; layout[4] = L.image_bytes; layout[5] = L.total_bytes;
     layout[6] = L.nblkA_padded; layout[7] = L.nblkB_padded; layout[8] = L.sm_image;
     layout[9] = G.im_para; layout[10] = G.im_dira; layout[11] = G.im_grpa; layout[12] = G.im_dirb; layout[13] = G.im_wbrec; layout[14] = G.im_parb;
     layout[15] = G.im_fcw; layout[16] = NWC; layout[17] = G.gpw; layout[18] = *reinterpret_cast<const uint32_t *>(out + G.im_fcwn); layout[19] = KPARTS;
-    layout[20] = G.na;
+    layout[20] = G.na; layout[21] = (uint32_t)fast_cvt;
     return r;
 }
 

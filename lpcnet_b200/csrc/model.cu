@@ -225,7 +225,7 @@ static int build_host_model(DeviceModel *m, HostModel &hm, const unsigned char *
     std::vector<std::vector<int>> grp(nwc);
     std::vector<int> load(nwc, 0);
     if (!is_float) {
-        // The compute warps do not carry the same load besides GRU_A: warps < 6*KPARTS also walk a (row group, K part) of the dense GRU_B
+        // The compute warps do not carry the same load besides GRU_A: warps < 6*KPARTS also walk a (row group, K part) of the GRU_B
         // input GEMV (blocks counted like GRU_A's), the last NFIN warps finish GRU_B (worth about `fin` blocks).  Starting the LPT from these
         // loads hands the heavier neuron groups to the warps with less GRU_B work (LPCNET_B200_LPT="<GRU_B block weight>,<finish cost>").
         int wgt = 1, fin = 48;
@@ -432,6 +432,12 @@ static int build_host_model(DeviceModel *m, HostModel &hm, const unsigned char *
             for (int o = 0; o < 8; o++) smax = std::max(smax, rs[o]);
         }
         const double bound = (bmax + dmax + cmax + 3 * emax) * 1.01 * (128.0 * 127.0) + 255.0 * smax + 2;
+        // Past int32 the two sides part ways: __float2int_rn saturates where the reference's cvtps2dq returns 0x80000000, and
+        // the integer sums wrap.  Refused like the pair constraint.
+        if (bound >= 2147483648.0) {
+            set_error("model: GRU_A pre-activations may reach %.4g accumulator units, beyond int32 (the reference's float->int32 conversion would overflow; the results would differ)", bound);
+            return -1;
+        }
         m->fast_cvt = bound < 4194304.0 * 0.99;
     }
     // ---------------- float flavour: second image for the neuron-per-lane kernel (small batches) ----------------
@@ -512,11 +518,11 @@ static int build_host_model(DeviceModel *m, HostModel &hm, const unsigned char *
 }
 
 // Test hook (no CUDA needed): build the shared-memory image on the host and hand it out.
-int debug_build_image(const unsigned char *blob, int len, unsigned char *out, size_t cap, SmemLayout *L, Geom *g)
+int debug_build_image(const unsigned char *blob, int len, unsigned char *out, size_t cap, SmemLayout *L, Geom *g, int *fast_cvt)
 {
     DeviceModel m; HostModel hm;
     if (build_host_model(&m, hm, blob, len, nullptr) != 0) return -1;
-    *L = m.L; *g = make_geom(m.na);
+    *L = m.L; *g = make_geom(m.na); *fast_cvt = m.fast_cvt;
     if (hm.img.size() > cap) { set_error("debug image: buffer too small"); return -1; }
     memcpy(out, hm.img.data(), hm.img.size());
     return (int)hm.img.size();

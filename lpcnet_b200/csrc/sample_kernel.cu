@@ -612,7 +612,7 @@ __device__ __forceinline__ void grub(const ComputeCtx &C, const SampleParams &P,
     (void)t; (void)warp; (void)rcp; (void)nxt; (void)xs_cur; (void)lc; (void)xs_nxt; (void)tile_r; (void)tile_z; (void)tile_h; (void)mb_full; (void)mb_empty; (void)lane;
     mbar_wait(smem_u32(smem + MB_X) + 8 * H, par);               // new quantised GRU_A state complete; candidate-gate tile dead: GRU_B scratch may use it
     TRACEC(P, trstep, 27, warp == 0 ? lane : 1);
-    // ---------------- GRU_B input GEMV (48 x 384 int8, dense): warp = (row group, K part) ----------------
+    // ---------------- GRU_B input GEMV (48 x 384 int8, block-sparse lists, dense or not): warp = (row group, K part) ----------------
     int *accB = reinterpret_cast<int *>(tile_hb + T_ACCB);
     float *hBs = reinterpret_cast<float *>(tile_hb + T_HBS);
     if (warp < NWB) {

@@ -100,11 +100,16 @@ def _sparse_pack(A, have_diag):
                 idx=np.array(idx, dtype=np.int32), AQ=AQ)
 
 
-def make_model(seed=1234, na=None, variant=""):
+def make_model(seed=1234, na=None, variant="", grub_keep=None, grua_keep=None, at_limits=None):
     """Returns (arrays_common, arrays_int8, arrays_float): ordered lists of (name, type, ndarray).
     na      : GRU_A units (default 384; other sizes are the `--grua-size` models of training_tf2/train_lpcnet.py)
     variant : "" | "clamp" (sampling tree biased towards large excitation so that the output runs into the +-32767 clamp of
-              lpcnet.c:265-269) | "dense" (GRU_A block densities 10/10/30 %)"""
+              lpcnet.c:265-269) | "dense" (GRU_A block densities 10/10/30 %)
+    The stress models (STRESS) change the block structure or the int8 values; with the three hooks None the model is unchanged:
+    grub_keep : rng -> bool [NA/4][6], the GRU_B input blocks kept per (column block, row group) (default: all, dense)
+    grua_keep : (rng, gate, q) -> bool [NA/4][NA/8], the GRU_A blocks kept, from the gate's quantised weights q [NA][NA]
+                (default: a uniform random mask of DENSITY)
+    at_limits : (rng, q, allowed) -> q, rewrites an int8 matrix [n_in][n_out] at the positions `allowed` (kept blocks)"""
     N_A = int(na or globals()["N_A"])
     DENSITY = (0.10, 0.10, 0.30) if variant == "dense" else globals()["DENSITY"]
     rng = np.random.default_rng(seed)
@@ -132,11 +137,21 @@ def make_model(seed=1234, na=None, variant=""):
     fl("gru_b_dense_feature_weights", rng.normal(0.0, 0.10, size=(COND, 3 * N_B)))
     fl("gru_b_dense_feature_bias", np.zeros(3 * N_B))
     qb_in = _quantized_matrix(rng, N_A, 3 * N_B, 0.09)
+    keep_b = np.ones((N_A // 4, 3 * N_B // 8), bool) if grub_keep is None else grub_keep(rng)
+    if grub_keep is not None:
+        qb_in = qb_in * np.repeat(np.repeat(keep_b, 4, axis=0), 8, axis=1)
+        for (jb, rg) in zip(*np.nonzero(keep_b)):            # a kept block stays non-empty (the dump drops all-zero blocks)
+            if not qb_in[jb * 4:jb * 4 + 4, rg * 8:rg * 8 + 8].any():
+                qb_in[jb * 4, rg * 8] = 1
+    if at_limits is not None:
+        qb_in = at_limits(rng, qb_in, np.repeat(np.repeat(keep_b, 4, axis=0), 8, axis=1))
     pk = _sparse_pack(qb_in / 128.0, have_diag=False)
     only8.append(("gru_b_weights", WEIGHT_TYPE_qweight, pk["w_int8"]))
     onlyf.append(("gru_b_weights", WEIGHT_TYPE_qweight, pk["w_float"]))
     common.append(("gru_b_weights_idx", WEIGHT_TYPE_int, pk["idx"]))
     qb_rec = _quantized_matrix(rng, N_B, 3 * N_B, 0.25)
+    if at_limits is not None:
+        qb_rec = at_limits(rng, qb_rec, np.ones(qb_rec.shape, bool))
     # dotp layout: reshape (in/4,4,out/8,8) -> transpose (2,0,3,1) = [out/8][in/4][8][4]  (dump_lpcnet.py:58-59)
     dot = qb_rec.reshape(N_B // 4, 4, 3 * N_B // 8, 8).transpose(2, 0, 3, 1).reshape(-1)
     only8.append(("gru_b_recurrent_weights", WEIGHT_TYPE_qweight, dot.astype(np.int8)))
@@ -185,13 +200,17 @@ def make_model(seed=1234, na=None, variant=""):
     # --- sparse GRU_A recurrent (dump_sparse_gru, dump_lpcnet.py:124-149)
     A = np.zeros((N_A, 3 * N_A))
     for k in range(3):
-        nblk = (N_A // 4) * (N_A // 8)
-        keep = nblk - int(round(nblk * (1 - DENSITY[k])))
-        chosen = rng.choice(nblk, size=keep, replace=False)
-        mask = np.zeros(nblk, dtype=bool)
-        mask[chosen] = True
-        mask = mask.reshape(N_A // 4, N_A // 8)
-        q = _quantized_matrix(rng, N_A, N_A, 0.17 if k < 2 else 0.13)
+        if grua_keep is None:
+            nblk = (N_A // 4) * (N_A // 8)
+            keep = nblk - int(round(nblk * (1 - DENSITY[k])))
+            chosen = rng.choice(nblk, size=keep, replace=False)
+            mask = np.zeros(nblk, dtype=bool)
+            mask[chosen] = True
+            mask = mask.reshape(N_A // 4, N_A // 8)
+            q = _quantized_matrix(rng, N_A, N_A, 0.17 if k < 2 else 0.13)
+        else:
+            q = _quantized_matrix(rng, N_A, N_A, 0.17 if k < 2 else 0.13)
+            mask = grua_keep(rng, k, q)
         # make sure every kept block is non-empty (dump drops all-zero blocks)
         full = np.repeat(np.repeat(mask, 4, axis=0), 8, axis=1)
         q = q * full
@@ -206,6 +225,8 @@ def make_model(seed=1234, na=None, variant=""):
             if not offd.any():
                 a, b_ = (0, 0) if (jb * 4 != ib * 8) else (1, 0)
                 q[jb * 4 + a, ib * 8 + b_] = 1
+        if at_limits is not None:                    # inside the kept blocks, off the diagonal (which the dump moves out as float)
+            q = at_limits(rng, q, full & ~np.eye(N_A, dtype=bool))
         A[:, k * N_A:(k + 1) * N_A] = q / 128.0
         # diagonal (kept outside the block structure, float, not quantised)
         d = rng.normal(0.25 if k == 2 else 0.1, 0.2, size=N_A)
@@ -412,6 +433,133 @@ VARIANTS = {
     "delay0": dict(delay=0),                              # FEATURES_DELAY 0: no look-ahead, LPC of the current frame (lpcnet.c:113-115)
     "na256e2e": dict(na=256, e2e=True, delay=0, gamma=0.95),
 }
+
+
+def _grub_split(rng):
+    """--grub-density 0.5 with --grub-density-split (training_tf2/train_lpcnet.py:46-78, SparsifyGRUB): the update and reset
+    rows sparse with unequal counts per row group, the candidate rows dense.  Row group 0 keeps one block (the second int8 K
+    part is empty), row group 2 three (a partial quad)."""
+    nin = N_A // 4
+    keep = np.ones((nin, 6), bool)
+    for rg, d in enumerate((0.15, 0.35, 0.20, 0.30)):
+        keep[:, rg] = rng.random(nin) < d
+    for rg, n in ((0, 1), (2, 3)):
+        keep[:, rg] = False
+        keep[rng.choice(nin, n, replace=False), rg] = True
+    return keep
+
+
+def _grub_even(rng):
+    """Every GRU_B row group keeps 42 column blocks at scattered positions: all lists alike but not dense; the int8 K parts
+    take 21 blocks each (5 full quads and a partial one)."""
+    keep = np.zeros((N_A // 4, 6), bool)
+    for rg in range(6):
+        keep[rng.choice(N_A // 4, 42, replace=False), rg] = True
+    return keep
+
+
+def _grua_skew(rng, gate, q):
+    """GRU_A blocks kept above one block-energy threshold per gate (Sparsify, training_tf2/lpcnet.py:96-116) of weights with
+    strong and weak neuron groups and inputs, so the list lengths are skewed; then the list shapes the kernels' walkers can get
+    wrong are forced on fixed row groups (the same groups in every gate):
+      0, 6, 7   empty          1, 2, 3   one, two and three blocks (partial quads)
+      4         8 blocks all of one (pos/4)&3 class (put_quads must repeat a class)
+      5, 8..15  include the last column block, pos = NA-4"""
+    nin, nout = N_A // 4, N_A // 8
+    e = (q.reshape(nin, 4, nout, 8).astype(np.float64) ** 2).sum(axis=(1, 3))
+    e *= np.exp(rng.normal(0.0, 1.2, size=(1, nout))) * np.exp(rng.normal(0.0, 0.6, size=(nin, 1)))
+    keep = e > np.quantile(e, 1.0 - (0.075, 0.075, 0.25)[gate])
+    for rg in (0, 6, 7):
+        keep[:, rg] = False
+    for rg, n in ((1, 1), (2, 2), (3, 3)):
+        keep[:, rg] = False
+        keep[rng.choice(nin, n, replace=False), rg] = True
+    keep[:, 4] = False
+    keep[4 * np.arange(2, 10) + (gate + 1) % 4, 4] = True
+    keep[nin - 1, 5] = True
+    keep[nin - 1, 8:16] = True
+    return keep
+
+
+LIMIT_PAIRS = ((64, 64), (-64, -64), (127, 1), (-1, -127), (-128, 0), (0, -128), (127, -128), (-128, 127))
+
+
+def _at_limits(rng, q, allowed, npairs=96):
+    """Puts `npairs` input pairs (rows 2k, 2k+1 of one column) at the limit the loader accepts (model.cu: |w0|+|w1| <= 128 for
+    same-sign pairs, any pair of int8 otherwise): same-sign pairs summing to 128, entries of -128 and the pair (127, -128).
+    Placed only where `allowed` (inside kept blocks, off the GRU_A diagonal)."""
+    q = q.copy()
+    cand = np.argwhere(allowed[0::2] & allowed[1::2])
+    for n, (k, c) in enumerate(cand[rng.choice(len(cand), size=min(npairs, len(cand)), replace=False)]):
+        q[2 * k, c], q[2 * k + 1, c] = LIMIT_PAIRS[n % len(LIMIT_PAIRS)]
+    return q
+
+
+def cvt_bound(arrays, na=N_A):
+    """Restates the loader's range proof for the conversion-free rounding of the GRU_A accumulators (model.cu): a bound, in
+    accumulator units (1/(128*127)), on every value the int8 GRU_A accumulators take.  `arrays`: {name: ndarray} of an int8 blob."""
+    a = lambda n: np.abs(np.asarray(arrays[n], np.float64))
+    cmax = (a("gru_a_dense_feature_bias") + a("gru_a_dense_feature_weights").reshape(COND, 3 * na).sum(axis=0)).max()
+    bmax = a("sparse_gru_a_subias").reshape(2, 3 * na)[1].max()
+    dmax = a("sparse_gru_a_recurrent_weights_diag").max()
+    emax = max(a("gru_a_embed_%s_weights" % nm).max() for nm in ("sig", "pred", "exc"))
+    w = np.abs(arrays["sparse_gru_a_recurrent_weights"].astype(np.int64)).reshape(-1, 8, 4).sum(axis=2)
+    idx, p, b, smax = arrays["sparse_gru_a_recurrent_weights_idx"], 0, 0, 0
+    for _ in range(3 * na // 8):
+        nb = int(idx[p]); p += nb + 1
+        smax = max(smax, int(w[b:b + nb].sum(axis=0).max()) if nb else 0); b += nb
+    return (bmax + dmax + cmax + 3 * emax) * 1.01 * (128.0 * 127.0) + 255.0 * smax + 2
+
+
+FAST_CVT_LIMIT = 4194304.0 * 0.99      # model.cu: conversion-free rounding while the bound stays below 0.99 * 2^22
+
+
+STRESS_SEED = 2100
+# Stress models (all GRU_A 384, the default header: the compiled reference builds A and B load them at run time).  name ->
+# make_model() hooks; "cvt" sets the loader's accumulator bound (cvt_bound) to that value by raising a few biases.
+STRESS = {
+    "grub_split": dict(grub_keep=_grub_split),
+    "grub_even":  dict(grub_keep=_grub_even),
+    "skew":       dict(grua_keep=_grua_skew),
+    "limits":     dict(at_limits=_at_limits),
+    "warm":       dict(cvt=FAST_CVT_LIMIT * (1 - 1e-3)),       # just inside the proof: conversion-free rounding, largest accumulators
+    "hot":        dict(cvt=FAST_CVT_LIMIT * (1 + 1e-3)),       # just outside: the loader falls back to the conversion unit
+    "overflow":   dict(cvt=2.0 ** 31 * 1.01),                  # accumulators could leave int32: the loader refuses the int8 blob
+}
+
+
+def make_stress_model(name):
+    """(arrays_common, arrays_int8, arrays_float) of STRESS[name]; each model has its own seed."""
+    kw = dict(STRESS[name])
+    target = kw.pop("cvt", None)
+    common, only8, onlyf = make_model(STRESS_SEED + list(STRESS).index(name), **kw)
+    if target is not None:
+        # the recurrent bias of the candidate gate of neuron group 0 (alternating signs, bias and su-bias alike) becomes the
+        # largest one, so that cvt_bound() == target: these neurons' accumulators are the largest the bound allows
+        arrs = {n: a for n, _, a in common + only8}
+        rows = 2 * N_A + np.arange(8)
+        sub, bias = arrs["sparse_gru_a_subias"], arrs["sparse_gru_a_bias"]
+        sub[1, rows] = bias[1, rows] = 0.0
+        rest = np.abs(sub[1]).max()
+        b = np.float32(rest + (target - cvt_bound(arrs)) / (1.01 * 128.0 * 127.0))
+        assert b > rest
+        sub[1, rows] = bias[1, rows] = b * np.where(np.arange(8) % 2, -1.0, 1.0).astype(np.float32)
+    return common, only8, onlyf
+
+
+def stress_arrays(name, kind="int8"):
+    common, only8, onlyf = make_stress_model(name)
+    return {n: a for n, _, a in common + (only8 if kind == "int8" else onlyf)}
+
+
+def generate_stress(out):
+    """Writes stress_<name>_{int8,float}.bin for every STRESS model into `out`."""
+    os.makedirs(out, exist_ok=True)
+    for name in STRESS:
+        common, only8, onlyf = make_stress_model(name)
+        write_blob(os.path.join(out, "stress_%s_int8.bin" % name), common + only8)
+        write_blob(os.path.join(out, "stress_%s_float.bin" % name), common + onlyf)
+    return out
 
 
 def generate(out, seed=1234, c_sources=True, na=None, e2e=False, delay=None, gamma=None):

@@ -36,6 +36,19 @@ def blob(kind="int8", tag=""):
     return open(os.path.join(gen_dir(tag), "model_%s.bin" % kind), "rb").read()
 
 
+STRESS_DIR = GEN + "_stress"
+
+
+@functools.lru_cache(None)
+def stress_blob(name, kind="int8"):
+    """Blob of one of gen_model.STRESS (kind int8 | float), generated into oracle/_gen_stress on first use."""
+    import gen_model
+    path = os.path.join(STRESS_DIR, "stress_%s_%s.bin" % (name, kind))
+    if not os.path.exists(path):
+        gen_model.generate_stress(STRESS_DIR)
+    return open(path, "rb").read()
+
+
 def model_config(tag=""):
     """(lpc_gamma, features_delay, end2end) the reference bakes into nnet_data.h for this variant."""
     import gen_model
@@ -105,33 +118,34 @@ def oracle_lib():
 
 
 @functools.lru_cache(None)
-def oracle_model(kind="int8", tag=""):
-    """CPU-restatement model for a blob flavour (int8 / float / int8_clamp) of a model variant (tag, gen_model.VARIANTS)."""
+def oracle_model(kind="int8", tag="", model_blob=None):
+    """CPU-restatement model for a blob flavour (int8 / float / int8_clamp) of a model variant (tag, gen_model.VARIANTS), or for
+    the explicit blob `model_blob` (with the variant's header settings)."""
     L = oracle_lib()
-    b = blob(kind, tag)
+    b = blob(kind, tag) if model_blob is None else model_blob
     gamma, delay, e2e = model_config(tag)
     m = L.oracle_model_create_ex(b, len(b), rcp_table().ctypes.data, gamma, delay, int(e2e), codebooks().ctypes.data)
     assert m, "oracle failed to parse the blob"
     return m
 
 
-def oracle_synth(features, kind="int8", nthreads=8, tag=""):
-    """features [n][T][20] float32 -> pcm [n][T*160] int16 via the CPU restatement."""
+def oracle_synth(features, kind="int8", nthreads=8, tag="", model_blob=None):
+    """features [n][T][20] float32 -> pcm [n][T*160] int16 via the CPU restatement (of `model_blob` when given)."""
     L = oracle_lib()
     f = np.ascontiguousarray(features, dtype=np.float32)
     n, T, stride = f.shape
     pcm = np.zeros((n, T * 160), dtype=np.int16)
-    L.oracle_synthesize_batch(oracle_model(kind, tag), f.ctypes.data, stride, n, T, nthreads, pcm.ctypes.data)
+    L.oracle_synthesize_batch(oracle_model(kind, tag, model_blob), f.ctypes.data, stride, n, T, nthreads, pcm.ctypes.data)
     return pcm
 
 
-def oracle_decode(packets, kind="int8", nthreads=8):
-    """packets [n][P][8] uint8 -> pcm [n][P*640] int16."""
+def oracle_decode(packets, kind="int8", nthreads=8, model_blob=None):
+    """packets [n][P][8] uint8 -> pcm [n][P*640] int16 (with `model_blob` when given)."""
     L = oracle_lib()
     p = np.ascontiguousarray(packets, dtype=np.uint8)
     n, P, _ = p.shape
     pcm = np.zeros((n, P * 640), dtype=np.int16)
-    L.oracle_decode_batch(oracle_model(kind), p.ctypes.data, n, P, nthreads, pcm.ctypes.data)
+    L.oracle_decode_batch(oracle_model(kind, "", model_blob), p.ctypes.data, n, P, nthreads, pcm.ctypes.data)
     return pcm
 
 
@@ -174,10 +188,11 @@ def ref_lib(build="A", tag=""):
     return L
 
 
-def ref_synth(features, build="A", tag="", kind=None, nthreads=None):
-    """features [n][T][stride] -> pcm [n][T*160] through the compiled reference (fresh lpcnet_create() per stream)."""
+def ref_synth(features, build="A", tag="", kind=None, nthreads=None, model_blob=None):
+    """features [n][T][stride] -> pcm [n][T*160] through the compiled reference (fresh lpcnet_create() per stream), loading
+    `model_blob` when given."""
     L = ref_lib(build, tag)
-    b = blob(kind or ("float" if build in ("B", "TB") else "int8"), tag)
+    b = blob(kind or ("float" if build in ("B", "TB") else "int8"), tag) if model_blob is None else model_blob
     f = np.ascontiguousarray(features, dtype=np.float32)
     n, T, stride = f.shape
     pcm = np.zeros((n, T * 160), dtype=np.int16)

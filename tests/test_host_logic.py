@@ -1,12 +1,11 @@
 """CPU tests (-m "not gpu") of the product's HOST logic: library loading, C-ABI surface, blob validation and the
 shared-memory image the per-sample kernel consumes (checked by replaying the kernel's block walk in numpy against
 a dense reconstruction of the model).  No compute entry point is called: without a GPU the engine must refuse."""
-import ctypes
 import os
 import re
-import numpy as np
 import pytest
 import helpers as H
+import image_replay as R
 import lpcnet_b200
 from lpcnet_b200 import api
 
@@ -46,12 +45,7 @@ def test_no_cpu_fallback_without_gpu(L):
     assert not L.lpcnet_decoder_create()
 
 
-def _image(L, blob):
-    out = np.zeros(256 * 1024, np.uint8)
-    lay = np.zeros(24, np.uint32)
-    L.lpcnet_b200_debug_image.argtypes = [ctypes.c_char_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    r = L.lpcnet_b200_debug_image(blob, len(blob), out.ctypes.data, out.size, lay.ctypes.data)
-    return r, out, lay
+_image = R.int8_image
 
 
 def test_blob_validation(L):
@@ -71,86 +65,14 @@ def test_smem_image_replays_to_the_dense_model(L):
     for GRU_B) and check the integer GEMV it encodes equals the dense int8 matrices of the model for random u8 inputs."""
     import gen_model
     common, only8, _ = gen_model.make_model()
-    arrs = {n: a for n, _, a in common + only8}
-    r, img, lay = _image(L, H.blob("int8"))
-    wA, metaA, wB, metaB, image_bytes, total, nA, nB, SM_IMAGE, PARA, DIRA, GRPA, DIRB, WBREC, PARB, FCW, NWC, GPW, FCN, KP = [int(v) for v in lay[:20]]
-    assert r == image_bytes and total <= 227 * 1024 and total == SM_IMAGE + image_bytes
-    img = img[:image_bytes]
-    rel = lambda o: o - SM_IMAGE
-
-    def dense_from_sparse(w8, idx, nrows, ncols):
-        M = np.zeros((nrows, ncols), np.int32); p = 0; wp = 0
-        for rg in range(nrows // 8):
-            nb = idx[p]; p += 1
-            for _ in range(nb):
-                pos = idx[p]; p += 1
-                M[rg * 8:rg * 8 + 8, pos:pos + 4] = w8[wp:wp + 32].reshape(8, 4); wp += 32
-        return M
-    MA = dense_from_sparse(arrs["sparse_gru_a_recurrent_weights"].astype(np.int32), arrs["sparse_gru_a_recurrent_weights_idx"], 1152, 384)
-    MB = dense_from_sparse(arrs["gru_b_weights"].astype(np.int32), arrs["gru_b_weights_idx"], 48, 384)
-    rng = np.random.default_rng(0)
-    x = rng.integers(0, 255, 384).astype(np.int32)
-    want_A, want_B = MA @ x, MB @ x
-
-    def xs_offset(c, s):
-        return c * 128 + (((((s >> 4) & 1) << 6) | ((s & 7) << 3)) ^ (((c & 1) << 6) | ((c & 2) << 4))) + ((s >> 3) & 1) * 4
-
-    def replay_quads(wq, mq, q0, nq):
-        """sum over quads q0..q0+nq of W[8 out][slot][4 in] . x[column block of the slot]; also counts bank-group clashes"""
-        acc = np.zeros(8, np.int64); clash = 0
-        for q in range(q0, q0 + nq):
-            classes = set()
-            for t in range(4):
-                e = int(mq[q, t]); c = e >> 7
-                assert e == xs_offset(c, 0) and c < 96
-                classes.add(c & 3)
-                acc += wq[q, :, t, :] @ x[4 * c:4 * c + 4]
-            clash += 4 - len(classes)
-        return acc, clash
-
-    dirA = img[DIRA:DIRA + NWC * GPW * 3 * 2 * 4].view(np.uint32).reshape(NWC, GPW, 3, 2)
-    grpA = img[GRPA:GRPA + NWC * GPW * 4].view(np.uint32).reshape(NWC, GPW)
-    parA = img[PARA:PARA + NWC * GPW * 3 * 16 * 4].view(np.float32).reshape(NWC, GPW, 3, 2, 8)
-    wAi = img[rel(wA):rel(wA) + nA * 128].view(np.int8).astype(np.int32).reshape(nA, 8, 4, 4)     # [quad][out][slot][in]
-    mA = img[rel(metaA):rel(metaA) + nA * 8].view(np.uint16).reshape(nA, 4)
-    assert sorted(grpA.reshape(-1).tolist()) == list(range(48))           # every neuron group owned exactly once
-    got = np.zeros(1152, np.int64)
-    loads = []; clashes = 0
-    for w in range(NWC):
-        tot = 0
-        for sl in range(GPW):
-            g = int(grpA[w, sl])
-            for q in range(3):
-                q0, nq = int(dirA[w, sl, q, 0]), int(dirA[w, sl, q, 1])
-                tot += nq
-                acc, cl = replay_quads(wAi, mA, q0, nq)
-                got[q * 384 + 8 * g:q * 384 + 8 * g + 8] += acc; clashes += cl
-                np.testing.assert_array_equal(parA[w, sl, q, 0], arrs["sparse_gru_a_subias"][1, q * 384 + 8 * g:q * 384 + 8 * g + 8])
-                np.testing.assert_array_equal(parA[w, sl, q, 1], arrs["sparse_gru_a_recurrent_weights_diag"][q * 384 + 8 * g:q * 384 + 8 * g + 8])
-        loads.append(tot)
-    np.testing.assert_array_equal(got, want_A)
+    s = R.replay_int8_image(L, H.blob("int8"), {n: a for n, _, a in common + only8})
+    loads, nA = s["loads"], s["nA"]
     # LPT balancing of the compute warps: the warps that also walk the GRU_B GEMV (first 12) and / or finish GRU_B (last 8) get lighter
     # GRU_A lists (model.cu), so the quad counts differ by class but stay within +-35 % of the mean
-    assert sum(loads) == nA and max(loads) <= 1.35 * (sum(loads) / NWC) and min(loads) >= 0.65 * (sum(loads) / NWC)
-    assert clashes <= 0.15 * 4 * nA                                       # slots of a quad mostly in different bank groups
-
-    dirB = img[DIRB:DIRB + 6 * KP * 2 * 4].view(np.uint32).reshape(6, KP, 2)
-    wBi = img[rel(wB):rel(wB) + nB * 128].view(np.int8).astype(np.int32).reshape(nB, 8, 4, 4)
-    mB = img[rel(metaB):rel(metaB) + nB * 8].view(np.uint16).reshape(nB, 4)
-    gotB = np.zeros(48, np.int64)
-    for rg in range(6):
-        for half in range(KP):
-            acc, cl = replay_quads(wBi, mB, int(dirB[rg, half, 0]), int(dirB[rg, half, 1]))
-            gotB[rg * 8:rg * 8 + 8] += acc
-            assert cl == 0                                                # dense rows: always conflict-free
-    np.testing.assert_array_equal(gotB, want_B)
-    # GRU_B recurrent block layout [out/8][in/4][8][4] and su-biases
-    np.testing.assert_array_equal(img[WBREC:WBREC + 768].view(np.int8), arrs["gru_b_recurrent_weights"])
-    np.testing.assert_array_equal(img[PARB:PARB + 96 * 4].view(np.float32), arrs["gru_b_subias"].reshape(-1))
-    fcw = img[FCW:FCW + FCN * 36 * 4].view(np.float32).reshape(FCN, 36)
-    np.testing.assert_array_equal(fcw[:, :32], arrs["dual_fc_weights"].reshape(256, 32)[:FCN])
-    np.testing.assert_array_equal(fcw[:, 32:34], arrs["dual_fc_bias"].reshape(2, 256).T[:FCN])
-    np.testing.assert_array_equal(fcw[:, 34:36], arrs["dual_fc_factor"].reshape(2, 256).T[:FCN])
+    assert max(loads) <= 1.35 * (nA / s["nwc"]) and min(loads) >= 0.65 * (nA / s["nwc"])
+    assert s["clashes"] <= 0.15 * 4 * nA                                  # slots of a quad mostly in different bank groups
+    assert s["clashesB"] == 0                                             # dense rows: always conflict-free
+    assert s["fcw_nodes"] == 64 and s["fast_cvt"] == 1
 
 
 def test_denser_model_trades_dual_fc_rows_for_weight_room(L, tmp_path, monkeypatch):
@@ -177,57 +99,8 @@ def test_float_neuron_image_replays_to_the_dense_model(L):
     [8 rows][4 cols]; walking it like the kernel must reproduce the dense float matrices (the weights are fp16-exact)."""
     import gen_model
     common, _, onlyf = gen_model.make_model()
-    arrs = {n: a for n, _, a in common + onlyf}
-    blob = H.blob("float")
-    out = np.zeros(300000, np.uint8); lay = (ctypes.c_uint32 * 32)()
-    L.lpcnet_b200_debug_image_n.argtypes = [ctypes.c_char_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
-    r = L.lpcnet_b200_debug_image_n(blob, len(blob), out.ctypes.data, out.size, lay)
-    wA, metaA, wB, metaB, image_bytes, total, nA, nB, IMG, NEUR, DIRA, PARA, DIRB, PARB, WBREC, FCW, dense = [int(v) for v in lay[:17]]
-    assert r == image_bytes and total <= 227 * 1024 and total == IMG + image_bytes
-    img = out[:image_bytes]
-    rel = lambda o: o - IMG
-
-    def dense_from_sparse(w, idx, nrows, ncols):
-        M = np.zeros((nrows, ncols), np.float64); p = 0; wp = 0
-        for rg in range(nrows // 8):
-            nb = idx[p]; p += 1
-            for _ in range(nb):
-                pos = idx[p]; p += 1
-                M[rg * 8:rg * 8 + 8, pos:pos + 4] = w[wp:wp + 32].reshape(4, 8).T; wp += 32      # blob block = [4 cols][8 rows]
-        return M
-    MA = dense_from_sparse(arrs["sparse_gru_a_recurrent_weights"].astype(np.float64), arrs["sparse_gru_a_recurrent_weights_idx"], 1152, 384)
-    MB = dense_from_sparse(arrs["gru_b_weights"].astype(np.float64), arrs["gru_b_weights_idx"], 48, 384)
-    neur = img[NEUR:NEUR + 768].view(np.uint16)
-    assert sorted(neur.tolist()) == list(range(384))                       # every neuron owned by exactly one lane
-    assert all((neur[8 * k:8 * k + 8] == neur[8 * k] + np.arange(8)).all() and neur[8 * k] % 8 == 0 for k in range(48))
-    dirA = img[DIRA:DIRA + 48 * 3 * 2 * 4].view(np.uint32).reshape(48, 3, 2)
-    blkA = img[rel(wA):rel(wA) + nA * 64].view(np.float16).astype(np.float64).reshape(nA, 8, 4)
-    mA = img[rel(metaA):rel(metaA) + nA * 2].view(np.uint16)
-    got = np.zeros((1152, 384))
-    for g in range(48):
-        for q in range(3):
-            b0, nb = int(dirA[g, q, 0]), int(dirA[g, q, 1])
-            for b in range(b0, b0 + nb):
-                pos = int(mA[b]) // 4
-                assert mA[b] % 16 == 0
-                got[q * 384 + 8 * g:q * 384 + 8 * g + 8, pos:pos + 4] += blkA[b]
-    np.testing.assert_array_equal(got, MA)
-    dirB = img[DIRB:DIRB + 48].view(np.uint32).reshape(6, 2)
-    blkB = img[rel(wB):rel(wB) + nB * 64].view(np.float16).astype(np.float64).reshape(nB, 8, 4)
-    mB = img[rel(metaB):rel(metaB) + nB * 2].view(np.uint16)
-    gotB = np.zeros((48, 384))
-    for rg in range(6):
-        b0, nb = int(dirB[rg, 0]), int(dirB[rg, 1])
-        for k, b in enumerate(range(b0, b0 + nb)):
-            pos = int(mB[b]) // 4
-            assert not dense or pos == 4 * k                               # dense flag: offsets are 16 * block index
-            gotB[rg * 8:rg * 8 + 8, pos:pos + 4] += blkB[b]
-    np.testing.assert_array_equal(gotB, MB)
-    para = img[PARA:PARA + 6 * 384 * 4].view(np.float32).reshape(3, 2, 384)
-    np.testing.assert_array_equal(para[:, 0], arrs["sparse_gru_a_bias"][1].reshape(3, 384))
-    np.testing.assert_array_equal(para[:, 1], arrs["sparse_gru_a_recurrent_weights_diag"].reshape(3, 384))
-    fcw = img[FCW:FCW + 256 * 36 * 4].view(np.float32).reshape(256, 36)
-    np.testing.assert_array_equal(fcw[:, :32], arrs["dual_fc_weights"].reshape(256, 32))
+    s = R.replay_float_image(L, H.blob("float"), {n: a for n, _, a in common + onlyf})
+    assert s["dense"] == 1 and s["chains"] == ["dense", "dense"]         # dense GRU_B input rows, in order
 
 
 def test_python_mirror_matches_reference_operator_names():
@@ -240,27 +113,9 @@ def test_python_mirror_matches_reference_operator_names():
 
 @pytest.mark.parametrize("tag,na", [("na128", 128), ("na256", 256), ("na256e2e", 256), ("", 384)])
 def test_images_of_all_gru_a_sizes_respect_the_kernel_budgets(L, tag, na):
-    """Every supported GRU_A size builds a shared-memory image that fits one SM; every neuron group is owned by exactly one compute
-    warp; and the quad arrays are followed by the readable slack that the pipelined GEMVs of sample_kernel.cu read past the end of a
-    stream (4 quads of weights, 6 meta entries)."""
-    r, img, lay = _image(L, H.blob("int8", tag))
-    wA, metaA, wB, metaB, image_bytes, total, nA, nB, SM_IMAGE, PARA, DIRA, GRPA, DIRB, WBREC, PARB, FCW, NWC, GPW, FCN, KP, NA = [int(v) for v in lay[:21]]
-    assert r == image_bytes and NA == na and NWC * GPW * 8 == na
-    assert total == SM_IMAGE + image_bytes and total <= 227 * 1024 and FCN in (8, 16, 32, 64)
-    img = img[:image_bytes]
-    dirA = img[DIRA:DIRA + NWC * GPW * 3 * 2 * 4].view(np.uint32).reshape(NWC, GPW, 3, 2)
-    grpA = img[GRPA:GRPA + NWC * GPW * 4].view(np.uint32).reshape(NWC, GPW)
-    dirB = img[DIRB:DIRB + 6 * KP * 2 * 4].view(np.uint32).reshape(6 * KP, 2)
-    assert sorted(grpA.reshape(-1).tolist()) == list(range(na // 8))
-    assert int(dirA[:, :, :, 1].sum()) == nA and int(dirB[:, 1].sum()) == nB
-    # the warp's lists are contiguous and in the order the kernel walks them: r0 h0 r1 h1 ... | z0 z1 ... (first quad of the warp = r of slot 0)
-    for w in range(NWC):
-        q = int(dirA[w, 0, 1, 0])
-        for sl in range(GPW):
-            for gate in (1, 2):
-                assert int(dirA[w, sl, gate, 0]) == q
-                q += int(dirA[w, sl, gate, 1])
-        for sl in range(GPW):
-            assert int(dirA[w, sl, 0, 0]) == q
-            q += int(dirA[w, sl, 0, 1])
-    assert metaA - wA >= (nA + 4) * 128 and wB - metaA >= (nA + 6) * 8 and metaB - wB >= (nB + 4) * 128 and total - metaB >= (nB + 6) * 8
+    """Every supported GRU_A size builds a shared-memory image that fits one SM and replays to the dense model; every neuron group
+    is owned by exactly one compute warp; and the quad arrays are followed by the readable slack that the pipelined GEMVs of
+    sample_kernel.cu read past the end of a stream (4 quads of weights, 6 meta entries)."""
+    import gen_model
+    common, only8, _ = gen_model.make_model(na=na)
+    R.replay_int8_image(L, H.blob("int8", tag), {n: a for n, _, a in common + only8}, na=na)
