@@ -272,6 +272,9 @@ LPCNET_EXPORT int lpcnet_b200_debug_image_n(const unsigned char *blob, int len, 
 /* Test hook: evaluate the engine's two implementations of the reference's _mm256_rcp_ps emulation (memory table /
  * table-free arithmetic) on n host floats. */
 LPCNET_EXPORT int lpcnet_b200_debug_rcp(LPCNetB200Batch *b, const float *x, float *out_table, float *out_arith, int n);
+/* Test hook: the conditioning network's full-range _mm256_rcp_ps emulation (zeros, denormals, infinities, NaN, |x| >= 2^126)
+ * and its tanh8_approx with the reference's NaN order on n host floats. */
+LPCNET_EXPORT int lpcnet_b200_debug_tanh_x86(LPCNetB200Batch *b, const float *x, float *out_rcp, float *out_tanh, int n);
 
 /* Default model / codebooks for the lpcnet.h single-stream API (the reference compiles its model in; this
  * library loads it at run time).  Also settable through env LPCNET_B200_MODEL / LPCNET_B200_CODEBOOKS (file

@@ -975,6 +975,30 @@ int lpcnet_b200_debug_rcp(LPCNetB200Batch *b, const float *x, float *out_table, 
     return 0;
 }
 
+// Test hook: the conditioning network's full-range _mm256_rcp_ps and tanh8_approx (devmath.cuh rcp_emul_x86 / tanh_approx_x86)
+// on n host floats.
+__global__ void debug_tanh_x86_kernel(const float *x, float *out_rcp, float *out_tanh, int n, const uint16_t *tab16)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    out_rcp[i] = rcp_emul_x86(x[i], tab16);
+    out_tanh[i] = tanh_approx_x86(x[i], tab16);
+}
+int lpcnet_b200_debug_tanh_x86(LPCNetB200Batch *b, const float *x, float *out_rcp, float *out_tanh, int n)
+{
+    if (!b || n <= 0) { set_error("debug_tanh_x86: bad arguments"); return -1; }
+    CK(cudaSetDevice(b->device));
+    float *d = nullptr;
+    CK(cudaMalloc(&d, (size_t)3 * n * sizeof(float)));
+    CK(cudaMemcpy(d, x, (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+    debug_tanh_x86_kernel<<<(n + 255) / 256, 256, 0, b->stream>>>(d, d + n, d + 2 * n, n, b->model.rcp16);
+    CK(cudaStreamSynchronize(b->stream));
+    CK(cudaMemcpy(out_rcp, d + n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(out_tanh, d + 2 * n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+    cudaFree(d);
+    return 0;
+}
+
 // Test hook (host only): image of the neuron-per-lane float kernel.  layout = {wA, metaA, wB, metaB, image_bytes, total_bytes,
 // nblkA, nblkB, fn_image, fni_neur, fni_dira, fni_para, fni_dirb, fni_parb, fni_wbrec, fni_fcw, dense flag, na}
 int lpcnet_b200_debug_image_n(const unsigned char *blob, int len, unsigned char *out, size_t cap, uint32_t *layout)

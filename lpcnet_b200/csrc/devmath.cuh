@@ -73,6 +73,36 @@ __device__ __forceinline__ float tanh_approx(float x, TAB tab16)
     return fmaxf(-1.f, fminf(1.f, num));
 }
 
+// _mm256_rcp_ps over the whole float range (captured on an Intel CPU, tests/golden/rcpps_edges.json): the sign passes through;
+// NaN comes back quieted; +-0 and denormals (read as zero) give +-inf; +-inf and every |x| >= 2^126, whose reciprocal would be
+// tiny, give +-0.  The table formula of rcp_emul covers the remaining biased exponents 1..252.
+__device__ __forceinline__ float rcp_emul_x86(float x, const uint16_t *__restrict__ tab16)
+{
+    const uint32_t u = __float_as_uint(x), a = u & 0x7FFFFFFFu, s = u & 0x80000000u;
+    if (a > 0x7F800000u) return __uint_as_float(u | 0x00400000u);
+    if (a < 0x00800000u) return __uint_as_float(s | 0x7F800000u);
+    if (a >= 0x7E800000u) return __uint_as_float(s);
+    return __uint_as_float(s | __float_as_uint(rcp_emul(__uint_as_float(a), tab16)));
+}
+
+// tanh8_approx for inputs of any size (the conditioning network, whose pre-activations follow the features without bound): from
+// |x| of about 5e7 the numerator is inf, from about 1.6e9 the reciprocal of the denominator is 0 and their product NaN, and
+// _mm256_min_ps / _mm256_max_ps return their SECOND operand when one is NaN, so the NaN comes out like the reference's (fminf /
+// fmaxf would clamp it to +-1).  The per-sample kernels keep tanh_approx: their pre-activations are bounded by the loader.
+__device__ __forceinline__ float tanh_approx_x86(float x, const uint16_t *__restrict__ tab16)
+{
+    const float N0 = 952.52801514f, N1 = 96.39235687f, N2 = 0.60863042f;
+    const float D0 = 952.72399902f, D1 = 413.36801147f, D2 = 11.88600922f;
+    float X2 = __fmul_rn(x, x);
+    float num = __fmaf_rn(__fmaf_rn(N2, X2, N1), X2, N0);
+    float den = __fmaf_rn(__fmaf_rn(D2, X2, D1), X2, D0);
+    num = __fmul_rn(num, x);
+    den = rcp_emul_x86(den, tab16);
+    num = __fmul_rn(num, den);
+    const float hi = 1.f < num ? 1.f : num;              // _mm256_min_ps(max_out, num)
+    return -1.f > hi ? -1.f : hi;                        // _mm256_max_ps(min_out, ...)
+}
+
 // sigmoid8_approx (vec_avx.h:421-440)
 template <typename TAB>
 __device__ __forceinline__ float sigmoid_approx(float x, TAB tab16)

@@ -358,7 +358,7 @@ __device__ void quantize_superframe(EncState &st, EncScratch &S, const EncTables
     __shared__ float diff[NB_BANDS];
     __shared__ int s_c0, s_mid, s_interp;
     if (tid == 0) {
-        int c0 = (int)floor(.5 + (double)(st.features[3][0] * 4));
+        int c0 = cvtt_x86(floor(.5 + (double)(st.features[3][0] * 4)));
         c0 = c0 < 63 ? c0 : 63; c0 = c0 > -64 ? c0 : -64;
         st.features[3][0] = c0 / 4.f;
         s_c0 = c0;
@@ -514,18 +514,20 @@ __device__ void superframe(EncState &st, EncScratch &S, const EncTables &T, bool
         if (voiced) {
             const float mean_pitch = sy / sw, max_a = mean_pitch / 32;
             best_a = MINF(max_a, MAXF(-max_a, best_a));
-            corr_id = (int)floor((double)((frame_corr - .3f) / .175f));
+            corr_id = cvtt_x86(floor((double)((frame_corr - .3f) / .175f)));
             if (quantize) frame_corr = 0.3875f + .175f * corr_id;
         } else {
             best_a = 0;
-            corr_id = (int)floor((double)(frame_corr / .075f));
+            corr_id = cvtt_x86(floor((double)(frame_corr / .075f)));
             if (quantize) frame_corr = 0.0375f + .075f * corr_id;
         }
         const float best_b = (sy - best_a * sx) / sw;
         const float center_pitch = best_b + 5.5f * best_a;
-        int main_pitch = (int)floor(.5 + 21. * 1.442695041 * log((double)(center_pitch / PMIN)));
+        // a superframe with excitation energy in one half-subframe only can make the slope 0/0: best_a and center_pitch are then
+        // NaN and the conversions must give INT_MIN like the reference's (modulation -3, packet field 1), not CUDA's 0
+        int main_pitch = cvtt_x86(floor(.5 + 21. * 1.442695041 * log((double)(center_pitch / PMIN))));
         main_pitch = main_pitch < 63 ? main_pitch : 63; main_pitch = main_pitch > 0 ? main_pitch : 0;
-        int modulation = (int)floor(.5 + (double)(16 * 7 * best_a / center_pitch));
+        int modulation = cvtt_x86(floor(.5 + (double)(16 * 7 * best_a / center_pitch)));
         modulation = modulation < 3 ? modulation : 3; modulation = modulation > -3 ? modulation : -3;
         for (int sub = 0; sub < 4; sub++) {
             if (quantize) {

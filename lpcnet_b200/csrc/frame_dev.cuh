@@ -1,10 +1,19 @@
 // frame_dev.cuh — warp-level device code shared by the 100 Hz kernels (frame_kernels.cu) and the analysis side (enc_kernels.cu):
-// the reference's 320-point mixed-radix FFT butterflies (kiss_fft.c) and lpc_from_cepstrum (freq.c:310-320).
+// the reference's 320-point mixed-radix FFT butterflies (kiss_fft.c), lpc_from_cepstrum (freq.c:310-320) and the x86 float->int
+// conversion of the (int)floor(...) sites.
 #pragma once
 #include <cstdint>
 #include "engine.h"
 
 namespace lpcnet_b200 {
+
+// (int)v of a double as x86's cvttsd2si computes it: truncation toward zero, and INT_MIN (the "integer indefinite" value) for
+// NaN and for anything outside int32.  CUDA's own conversion returns 0 for NaN and saturates out-of-range values, which the
+// clamps after the reference's (int)floor(...) sites would turn into a different index.
+__device__ __forceinline__ int cvtt_x86(double v)
+{
+    return (v > -2147483649.0 && v < 2147483648.0) ? (int)v : (int)0x80000000u;
+}
 
 struct c32 { float r, i; };
 #define CMUL(m_, a_, b_) do { (m_).r = (a_).r * (b_).r - (a_).i * (b_).i; (m_).i = (a_).r * (b_).i + (a_).i * (b_).r; } while (0)

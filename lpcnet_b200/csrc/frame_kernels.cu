@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(GT_THREADS) frame_gemm_kernel(const GemmArgs a
 #pragma unroll
             for (int e = 0; e < 4; e++) {
                 float y = acc[4 * h + e][c];
-                if (TANH) y = tanh_approx(y, a.rcp16);
+                if (TANH) y = tanh_approx_x86(y, a.rcp16);
                 v[e] = zero ? 0.f : y;
             }
             *reinterpret_cast<float4 *>(yp + 32 * h) = make_float4(v[0], v[1], v[2], v[3]);
@@ -174,8 +174,9 @@ __global__ void __launch_bounds__(128) frame_assemble_kernel(const FrameIoArgs a
         float v;
         if (j < NB_FEAT) v = ft[j];
         else {
-            // pitch = (int)floor(.1 + 50*features[NB_BANDS]+100): 50*f is a float product, the sums are double
-            int p = (int)floor((.1 + (double)__fmul_rn(50.f, ft[NB_BANDS])) + 100.0);
+            // pitch = (int)floor(.1 + 50*features[NB_BANDS]+100): 50*f is a float product, the sums are double; past int32
+            // (f above about 4.3e7, inf) and for NaN x86 gives INT_MIN, which the clamp turns into 33
+            int p = cvtt_x86(floor((.1 + (double)__fmul_rn(50.f, ft[NB_BANDS])) + 100.0));
             p = min(255, max(33, p));
             v = __ldg(&a.embed_pitch[p * PITCH_EMBED + (j - NB_FEAT)]);
         }

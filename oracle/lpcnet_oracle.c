@@ -193,11 +193,18 @@ static void build_tables(OModel *m)
 }
 
 /* ------------------------------------------------------------------ scalar primitives ------------------------------------------------------------------ */
+/* over the whole float range (tests/golden/rcpps_edges.json): sign passed through, NaN quieted, +-0 and denormals -> +-inf,
+ * +-inf and |x| >= 2^126 (tiny reciprocal, flushed) -> +-0; the table covers biased exponents 1..252 */
 static inline float rcp_emul(const OModel *m, float x)
 {
     union { float f; uint32_t u; } in, out;
+    uint32_t a, s;
     in.f = x;
-    out.u = m->rcp[(in.u >> 12) & 0x7FF] - ((in.u & 0x7F800000u) - 0x3F800000u);
+    a = in.u & 0x7FFFFFFFu; s = in.u & 0x80000000u;
+    if (a > 0x7F800000u) out.u = in.u | 0x00400000u;
+    else if (a < 0x00800000u) out.u = s | 0x7F800000u;
+    else if (a >= 0x7E800000u) out.u = s;
+    else out.u = s | (m->rcp[(a >> 12) & 0x7FF] - ((a & 0x7F800000u) - 0x3F800000u));
     return out.f;
 }
 static inline float minps(float a, float b) { return a < b ? a : b; }   /* _mm_min_ps(a,b): a<b ? a : b */
@@ -438,15 +445,20 @@ static void rc2lpc(float *lpc, const float *rc)                      /* lpcnet.c
     for (i = 0; i < LPC_ORDER; i++) lpc[i] = tmp[i];
 }
 
+/* row of the pitch embedding (lpcnet.c:93-94); an x86 build: NaN and values past int32 convert to INT_MIN, clamped to 33 */
+int oracle_pitch_index(float f)
+{
+    int pitch = (int)floor(.1 + 50 * f + 100);
+    return pitch > 255 ? 255 : (pitch < 33 ? 33 : pitch);          /* IMIN(255, IMAX(33, pitch)) */
+}
+
 static void run_frame_network(OState *st, const float *features)     /* lpcnet.c:82-120 */
 {
     const OModel *m = st->m;
     const int N_A = m->na, delay = m->features_delay;
     float in[FRAME_IN], conv1_out[COND], conv2_out[COND], dense1_out[COND], condition[COND];
     float *lpc = st->lpc;
-    int pitch, i;
-    pitch = (int)floor(.1 + 50 * features[NB_BANDS] + 100);
-    pitch = pitch > 255 ? 255 : (pitch < 33 ? 33 : pitch);        /* IMIN(255, IMAX(33, pitch)) */
+    int pitch = oracle_pitch_index(features[NB_BANDS]), i;
     memcpy(in, features, sizeof(float) * NB_FEATURES);
     memcpy(in + NB_FEATURES, m->embed_pitch + pitch * PITCH_EMBED, sizeof(float) * PITCH_EMBED);
     conv1d(m, conv1_out, st->conv1_state, m->conv1_w, m->conv1_b, FRAME_IN, COND, in);
@@ -781,6 +793,7 @@ void oracle_get_tables(const OModel *m, float *tw /*640*/, int *bitrev /*320*/, 
     memcpy(logit, m->logit, sizeof(m->logit)); memcpy(u2l, m->ulaw2lin_tab, sizeof(m->ulaw2lin_tab));
 }
 float oracle_tanh(const OModel *m, float x) { return tanh_a(m, x); }
+float oracle_rcp(const OModel *m, float x) { return rcp_emul(m, x); }
 float oracle_sigmoid(const OModel *m, float x) { return sigmoid_a(m, x); }
 int oracle_lin2ulaw(float x) { return lin2ulaw(x); }
 void oracle_get_state(const OState *st, float *gru_a /*384*/, float *gru_b /*16*/, float *last_sig /*16*/, int *misc /*[last_exc, frame_count]*/, uint32_t *rng /*4*/)

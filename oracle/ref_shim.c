@@ -28,6 +28,17 @@ void ref_rcp_table(uint32_t *out)
 }
 
 float ref_rcp(float x) { return _mm_cvtss_f32(_mm_rcp_ss(_mm_set_ss(x))); }
+/* _mm256_rcp_ps (the instruction inside tanh8_approx / sigmoid8_approx, vec_avx.h:408,437) on n floats */
+void ref_rcp8(const float *x, float *out, int n)
+{
+    int i, j;
+    for (i = 0; i < n; i += 8) {
+        float in[8] = {0}, o[8];
+        for (j = 0; j < 8 && i + j < n; j++) in[j] = x[i + j];
+        _mm256_storeu_ps(o, _mm256_rcp_ps(_mm256_loadu_ps(in)));
+        for (j = 0; j < 8 && i + j < n; j++) out[i + j] = o[j];
+    }
+}
 int ref_lin2ulaw(float x) { return lin2ulaw(x); }
 float ref_ulaw2lin(float u) { return ulaw2lin(u); }
 void ref_activation(float *out, const float *in, int n, int act) { compute_activation(out, in, n, act); }

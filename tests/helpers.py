@@ -114,6 +114,12 @@ def oracle_lib():
     L.oracle_enc_single_frame_features.argtypes = [c_p, c_p, c_p]
     L.oracle_enc_encode.argtypes = [c_p, c_p, c_p]
     L.oracle_enc_compute_features.argtypes = [c_p, c_p, c_p]
+    L.oracle_enc_single_frame_features_float.argtypes = [c_p, c_p, c_p]
+    L.oracle_enc_last_best_a.restype = ctypes.c_float
+    L.oracle_enc_last_best_a.argtypes = [c_p]
+    L.oracle_pitch_index.argtypes = [ctypes.c_float]
+    L.oracle_rcp.restype = ctypes.c_float
+    L.oracle_rcp.argtypes = [c_p, ctypes.c_float]
     return L
 
 
@@ -167,6 +173,8 @@ def ref_lib(build="A", tag=""):
     L.ref_frame_network.argtypes = [ctypes.c_char_p, ctypes.c_int, c_p, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
     L.ref_rcp.restype = ctypes.c_float
     L.ref_rcp.argtypes = [ctypes.c_float]
+    if hasattr(L, "ref_rcp8"):                  # a reference compiled before the shim had it lacks the symbol
+        L.ref_rcp8.argtypes = [c_p, c_p, ctypes.c_int]
     L.ref_ulaw2lin.restype = ctypes.c_float
     L.ref_ulaw2lin.argtypes = [ctypes.c_float]
     L.ref_lin2ulaw.argtypes = [ctypes.c_float]
@@ -283,16 +291,64 @@ def ref_features4(pcm, build="A"):
 
 # ---- CPU restatement of the analysis side (oracle/lpcnet_enc_oracle.inc), one fresh state per stream ----
 def oracle_features(pcm):
+    """pcm [n][T*160] int16 (or float32: the _float entry point) -> features [n][T][36]."""
     L = oracle_lib()
-    p = np.ascontiguousarray(pcm, dtype=np.int16)
+    is_float = np.asarray(pcm).dtype == np.float32
+    p = np.ascontiguousarray(pcm, dtype=np.float32 if is_float else np.int16)
+    fn = L.oracle_enc_single_frame_features_float if is_float else L.oracle_enc_single_frame_features
     n, T = p.shape[0], p.shape[1] // 160
     out = np.zeros((n, T, 36), np.float32)
     for s in range(n):
         e = L.oracle_enc_create(None)
         for t in range(T):
-            L.oracle_enc_single_frame_features(e, p[s, t * 160:].ctypes.data, out[s, t].ctypes.data)
+            fn(e, p[s, t * 160:].ctypes.data, out[s, t].ctypes.data)
         L.oracle_enc_destroy(e)
     return out
+
+
+def oracle_encode_slopes(pcm):
+    """pcm [P*640] int16 of one stream -> (packets [P][8], pitch slope best_a of each superframe before the voicing decision)."""
+    L = oracle_lib()
+    p = np.ascontiguousarray(pcm, dtype=np.int16)
+    P = p.shape[0] // 640
+    cb = codebooks()
+    out, slopes = np.zeros((P, 8), np.uint8), np.zeros(P, np.float32)
+    e = L.oracle_enc_create(cb.ctypes.data)
+    for k in range(P):
+        L.oracle_enc_encode(e, p[k * 640:].ctypes.data, out[k].ctypes.data)
+        slopes[k] = L.oracle_enc_last_best_a(e)
+    L.oracle_enc_destroy(e)
+    return out, slopes
+
+
+def oracle_frame_taps(features, kind="int8"):
+    """features [n][T][stride] -> (gru_a cond [n][T][3*na], gru_b cond [n][T][48], weighted lpc [n][T][16]) of the CPU
+    restatement's run_frame_network on a fresh state per stream."""
+    L = oracle_lib()
+    f = np.ascontiguousarray(features, dtype=np.float32)
+    n, T, _ = f.shape
+    m = oracle_model(kind)
+    na = L.oracle_model_na(m)
+    ga, gb, lpc = np.zeros((n, T, 3 * na), np.float32), np.zeros((n, T, 48), np.float32), np.zeros((n, T, 16), np.float32)
+    for s in range(n):
+        st = L.oracle_state_create(m)
+        for t in range(T):
+            L.oracle_frame_network(st, f[s, t].ctypes.data, ga[s, t].ctypes.data, gb[s, t].ctypes.data, lpc[s, t].ctypes.data)
+        L.oracle_state_destroy(st)
+    return ga, gb, lpc
+
+
+def ref_frame_taps(features, build="A"):
+    """The same taps from the compiled reference's run_frame_network (ref_shim.c ref_frame_network)."""
+    L = ref_lib(build)
+    b = blob("float" if build in ("B", "TB") else "int8")
+    f = np.ascontiguousarray(features, dtype=np.float32)
+    n, T, stride = f.shape
+    na = 384
+    ga, gb, lpc = np.zeros((n, T, 3 * na), np.float32), np.zeros((n, T, 48), np.float32), np.zeros((n, T, 16), np.float32)
+    for s in range(n):
+        assert L.ref_frame_network(b, len(b), f[s].ctypes.data, stride, T, ga[s].ctypes.data, gb[s].ctypes.data, lpc[s].ctypes.data) == 0
+    return ga, gb, lpc
 
 
 def oracle_encode(pcm, features4=False):
