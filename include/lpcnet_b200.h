@@ -124,21 +124,28 @@ LPCNET_EXPORT int lpcnet_b200_batch_synthesize_device_ex(LPCNetB200Batch *b, con
 /* == the other internal entry points the reference's PLC uses (src/lpcnet_private.h:125-133), batched ==
  * run_frame_network (src/lpcnet.c:82-120) only: advances the 100 Hz state, keeps the last frame's conditioning */
 LPCNET_EXPORT int lpcnet_b200_batch_run_frame_network(LPCNetB200Batch *b, const float *features, int nframes, int feature_stride);
-/* lpcnet_synthesize_tail_impl (src/lpcnet.c:235-271): `samples` samples with the conditioning of the last frame-network run;
- * pcm [n_streams][samples] */
+/* lpcnet_synthesize_tail_impl (src/lpcnet.c:235-271): `samples` samples with the conditioning and LPC of the last
+ * _synthesize* or _run_frame_network call; pcm [n_streams][samples].  As in the reference, what the tail reads is per-stream
+ * state: a flush leaves it as it was; a reset zeroes it for the streams it resets (so a tail right after one gives zeros);
+ * a snapshot restore brings back what the snapshot saved.  After an _import_state the call is refused until the next
+ * _synthesize* or _run_frame_network call: the exported state carries no conditioning. */
 LPCNET_EXPORT int lpcnet_b200_batch_synthesize_tail(LPCNetB200Batch *b, int samples, short *pcm, int preload);
 /* run_frame_network_deferred / run_frame_network_flush (src/lpcnet.c:122-144): queue one feature frame per stream
- * (features [n_streams][feature_stride], at most 4 queued, older ones drop out) / run the frame network over the queue */
+ * (features [n_streams][feature_stride], at most 4 queued, older ones drop out) / run the frame network over the queue.
+ * Each stream has its own queue: a reset or an import of a stream empties it, and the flush runs only the frames the stream
+ * queued since.  The flush's conditioning is discarded; a later tail still reads that of the last frame-network run. */
 LPCNET_EXPORT int lpcnet_b200_batch_frame_network_deferred(LPCNetB200Batch *b, const float *features, int feature_stride);
 LPCNET_EXPORT int lpcnet_b200_batch_frame_network_flush(LPCNetB200Batch *b);
 
 /* == state by value ==  The reference's PLC copies `LPCNetState` structs to roll back speculative synthesis
- * (src/lpcnet_plc.c:216-230).  One stream <-> opaque host blob of lpcnet_b200_batch_state_size() bytes (everything
- * lpcnet_reset() clears: GRU states, signal history, conv/LPC delay lines, decoder memory, RNG, frame counter): */
+ * (src/lpcnet_plc.c:216-230).  One stream <-> opaque host blob of lpcnet_b200_batch_state_size() bytes (GRU states, signal
+ * history, conv/LPC delay lines, decoder memory, RNG, frame counter).  The blob leaves out the conditioning a tail reads and
+ * the deferred queue: exporting a stream with queued frames is refused, and an import empties the stream's queue and
+ * refuses tails until the next frame-network run. */
 LPCNET_EXPORT int lpcnet_b200_batch_state_size(const LPCNetB200Batch *b);
 LPCNET_EXPORT int lpcnet_b200_batch_export_state(LPCNetB200Batch *b, int stream, void *buf);
 LPCNET_EXPORT int lpcnet_b200_batch_import_state(LPCNetB200Batch *b, int stream, const void *buf);
-/* ... and the whole batch, device to device: */
+/* ... and the whole batch, device to device, including what a tail reads and the deferred queues: */
 LPCNET_EXPORT LPCNetB200Snapshot *lpcnet_b200_batch_snapshot_create(LPCNetB200Batch *b);
 LPCNET_EXPORT void lpcnet_b200_batch_snapshot_destroy(LPCNetB200Snapshot *s);
 LPCNET_EXPORT int lpcnet_b200_batch_snapshot_save(LPCNetB200Batch *b, LPCNetB200Snapshot *s);

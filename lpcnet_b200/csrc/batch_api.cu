@@ -22,6 +22,10 @@ using namespace lpcnet_b200;
 
 static const int CHUNK = FRAME_CHUNK;   // frames of conditioning buffered per sample-kernel launch
 static const int DEFER_MAX = 4;     // MAX_FEATURE_BUFFER_SIZE (lpcnet_private.h:26): conv1.kernel_size + conv2.kernel_size - 2
+// One more conditioning frame past the chunk slots: the frame a tail reads once a flush, a reset or a restore has put it there.
+// It plays the part of the reference's gru_a_condition / gru_b_condition / lpc, which a flush does not touch (lpcnet.c:134-144).
+// Its LPC lives in lpc_raw entry CHUNK + 2, past the entries 0..CHUNK+1 a chunk writes.
+static const int TAIL_SLOT = CHUNK;
 
 // the sample-rate part of the per-stream state (resettable part of struct LPCNetState), structure of arrays
 struct SampleState { float *hA, *hB, *last_sig, *deemph; int *last_exc; uint32_t *rng; };
@@ -33,15 +37,19 @@ struct LPCNetB200Batch {
     SampleState ss;
     SampleState shadow;                           // scratch copy for frames in which only SOME streams are still in their silent warm-up
     int *d_nsil;                                  // [n] silent frames of each stream in the segment being processed (mixed segments only)
+    FrameState fshadow;                           // scratch copy of the 100 Hz state for flushes in which only SOME streams have queued frames
+    int *d_keep;                                  // [DEFER_MAX][n] 1 = the stream sits that queued frame out (such flushes only)
     std::vector<int> *fc;                         // host mirror of fs.frame_count
-    // work buffers
+    // work buffers: CHUNK chunk slots + TAIL_SLOT
     float *condA, *condB, *lpc_raw;
-    int cond_last;                                // chunk position of the most recent frame-network output (for the *_tail entry point), -1 = none
+    int cond_last;                                // slot of the conditioning a tail reads (a chunk position or TAIL_SLOT); -1 = none since an import
     float *d_features; size_t d_features_cap;     // staging for host-pointer calls / decoder output
     short *d_pcm; size_t d_pcm_cap;
     uint8_t *d_packets; size_t d_packets_cap;
     float *d_state; size_t d_state_cap;           // staging for export/import of one stream's state
-    std::vector<float> *deferred; int deferred_fill;   // run_frame_network_deferred buffer: [DEFER_MAX][n][20] on the host
+    // run_frame_network_deferred queue: [DEFER_MAX][n][20] on the host, deferred_fill frames long.  Stream s has queued the LAST
+    // (*dfill)[s] <= deferred_fill of them (a reset or an import empties one stream's queue, lpcnet.c:174-182).
+    std::vector<float> *deferred; int deferred_fill; std::vector<int> *dfill;
     cudaStream_t stream;
     // Ordering of the engine state across CUDA streams: every call that enqueues work records `order_ev` on the stream it
     // used; the next call makes ITS stream wait for that event first (and host-side readers synchronise on it).  A caller
@@ -182,12 +190,24 @@ __global__ void state_pack_kernel(StateView v, int s, float *buf, int dir)
     mv(reinterpret_cast<float *>(v.ss.rng), n, 4, s);
 }
 
-// lpcnet_reset (lpcnet.c:174-182) for the listed streams (ids == NULL: all n streams); signal_only = lpcnet_reset_signal (lpcnet.c:226-233)
-__global__ void reset_streams_kernel(StateView v, const int *ids, int count, uint4 seed, int signal_only)
+// One frame of conditioning as the per-sample kernel reads it: condA (int8 [3 gates][n][na + 8], float [n][3*na]), condB [n][3*NB],
+// raw LPC [n][16]
+struct CondFrame { float *A, *B, *L; };
+
+// lpcnet_reset (lpcnet.c:174-182) for the listed streams (ids == NULL: all n streams); signal_only = lpcnet_reset_signal (lpcnet.c:226-233).
+// A full reset also zeroes the streams' entries of `tail` (the reference clears gru_a_condition, gru_b_condition and lpc), if given.
+__global__ void reset_streams_kernel(StateView v, const int *ids, int count, uint4 seed, int signal_only, CondFrame tail, int a_float)
 {
     const int k = blockIdx.x;
     if (k >= count) return;
     const size_t n = v.n, s = ids ? ids[k] : k;
+    if (!signal_only && tail.A) {
+        const int na = v.na;
+        if (a_float) for (int i = threadIdx.x; i < 3 * na; i += blockDim.x) tail.A[s * 3 * na + i] = 0.f;
+        else for (int i = threadIdx.x; i < 3 * na; i += blockDim.x) tail.A[((i / na) * n + s) * (na + 8) + i % na] = 0.f;
+        for (int i = threadIdx.x; i < 3 * NB; i += blockDim.x) tail.B[s * 3 * NB + i] = 0.f;
+        for (int i = threadIdx.x; i < LPC_ORDER; i += blockDim.x) tail.L[s * LPC_ORDER + i] = 0.f;
+    }
     for (int i = threadIdx.x; i < v.na; i += blockDim.x) v.ss.hA[i * n + s] = 0.f;
     for (int i = threadIdx.x; i < NB; i += blockDim.x) { v.ss.hB[i * n + s] = 0.f; v.ss.last_sig[i * n + s] = 0.f; }
     if (threadIdx.x == 0) { v.ss.deemph[s] = 0.f; v.ss.last_exc[s] = 128; }      // last_exc = lin2ulaw(0.f) = 128 (lpcnet.c:180)
@@ -216,7 +236,72 @@ __global__ void restore_silent_kernel(SampleState cur, SampleState old, const in
     for (int i = threadIdx.x; i < spf; i += blockDim.x) pcm[(size_t)s * pcm_stride + i] = 0;
 }
 
+// after a one-frame launch of a flush: streams that sit the frame out (keep[s]) get their 100 Hz state back from the shadow copy
+__global__ void keep_frame_state_kernel(FrameState cur, FrameState old, const int *keep, int n)
+{
+    const int s = blockIdx.x;
+    if (s >= n || !keep[s]) return;
+    for (int i = threadIdx.x; i < 2 * FRAME_IN; i += blockDim.x) cur.conv1_state[(size_t)s * 2 * FRAME_IN + i] = old.conv1_state[(size_t)s * 2 * FRAME_IN + i];
+    for (int i = threadIdx.x; i < 2 * COND; i += blockDim.x) cur.conv2_state[(size_t)s * 2 * COND + i] = old.conv2_state[(size_t)s * 2 * COND + i];
+    for (int i = threadIdx.x; i < LPC_ORDER; i += blockDim.x) {
+        cur.lpc_carry[(size_t)s * LPC_ORDER + i] = old.lpc_carry[(size_t)s * LPC_ORDER + i];
+        cur.lpc_carry[((size_t)n + s) * LPC_ORDER + i] = old.lpc_carry[((size_t)n + s) * LPC_ORDER + i];
+    }
+    if (threadIdx.x == 0) cur.frame_count[s] = old.frame_count[s];
+}
+
 static StateView view_of(LPCNetB200Batch *b) { return StateView{b->n, b->model.na, b->ss, b->fs}; }
+
+static size_t condA_floats(const LPCNetB200Batch *b) { return condA_frame_floats(b->model.is_float != 0, b->n, b->model.na); }
+// the conditioning the per-sample kernel reads for the frame in slot `pos`; frame f of a chunk reads lpc_raw entry f + 2 - d
+// (frame_kernels.cu), TAIL_SLOT its own entry
+static CondFrame frame_at(const LPCNetB200Batch *b, int pos)
+{
+    const size_t n = b->n;
+    const int d = b->model.cfg.end2end ? 0 : b->model.cfg.features_delay;
+    const size_t e = pos == TAIL_SLOT ? CHUNK + 2 : pos + 2 - d;
+    return CondFrame{b->condA + pos * condA_floats(b), b->condB + pos * n * 3 * NB, b->lpc_raw + e * n * LPC_ORDER};
+}
+static int copy_cond_frame(const LPCNetB200Batch *b, const CondFrame &dst, const CondFrame &src, cudaStream_t st)
+{
+    CK(cudaMemcpyAsync(dst.A, src.A, sizeof(float) * condA_floats(b), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst.B, src.B, sizeof(float) * b->n * 3 * NB, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst.L, src.L, sizeof(float) * b->n * LPC_ORDER, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+// move the frame a tail reads into TAIL_SLOT, out of the chunk slots the next frame-network run overwrites
+static int park_tail(LPCNetB200Batch *b, cudaStream_t st)
+{
+    if (b->cond_last < 0 || b->cond_last == TAIL_SLOT) return 0;
+    if (copy_cond_frame(b, frame_at(b, TAIL_SLOT), frame_at(b, b->cond_last), st)) return -1;
+    b->cond_last = TAIL_SLOT;
+    return 0;
+}
+
+static bool alloc_frame_state(FrameState *fs, size_t n)
+{
+    bool ok = true;
+    auto al = [&](void **p, size_t bytes) { if (ok && cudaMalloc(p, bytes) != cudaSuccess) ok = false; };
+    al((void **)&fs->conv1_state, sizeof(float) * 2 * FRAME_IN * n); al((void **)&fs->conv2_state, sizeof(float) * 2 * COND * n);
+    al((void **)&fs->lpc_carry, sizeof(float) * 2 * LPC_ORDER * n); al((void **)&fs->vq_mem, sizeof(float) * NB_BANDS * n);
+    al((void **)&fs->frame_count, sizeof(int) * n);
+    return ok;
+}
+static void free_frame_state(FrameState *fs)
+{
+    void *p[] = {fs->conv1_state, fs->conv2_state, fs->lpc_carry, fs->vq_mem, fs->frame_count};
+    for (void *q : p) if (q) cudaFree(q);
+    fs->conv1_state = fs->conv2_state = fs->lpc_carry = fs->vq_mem = nullptr; fs->frame_count = nullptr;
+}
+static int copy_frame_state(const FrameState &dst, const FrameState &src, size_t n, cudaStream_t st)
+{
+    CK(cudaMemcpyAsync(dst.conv1_state, src.conv1_state, sizeof(float) * 2 * FRAME_IN * n, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst.conv2_state, src.conv2_state, sizeof(float) * 2 * COND * n, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst.lpc_carry, src.lpc_carry, sizeof(float) * 2 * LPC_ORDER * n, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst.vq_mem, src.vq_mem, sizeof(float) * NB_BANDS * n, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(dst.frame_count, src.frame_count, sizeof(int) * n, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
 
 static int alloc_sample_state(SampleState *ss, size_t n, int na)
 {
@@ -266,14 +351,18 @@ static int reset_impl(LPCNetB200Batch *b, const int *ids, int count, int signal_
         CK(cudaMalloc((void **)&d_ids, sizeof(int) * count));
         CK(cudaMemcpyAsync(d_ids, ids, sizeof(int) * count, cudaMemcpyHostToDevice, b->stream));
     }
-    reset_streams_kernel<<<count, 128, 0, b->stream>>>(view_of(b), d_ids, count, make_uint4(seed[0], seed[1], seed[2], seed[3]), signal_only);
+    // a full reset of every stream leaves the zeroed TAIL_SLOT as what a tail reads; a per-stream one zeroes the streams' part of
+    // the current tail frame (none since an import: tails stay refused until the next frame-network run)
+    if (!signal_only && !ids) b->cond_last = TAIL_SLOT;
+    const CondFrame tail = b->cond_last >= 0 ? frame_at(b, b->cond_last) : CondFrame{nullptr, nullptr, nullptr};
+    reset_streams_kernel<<<count, 128, 0, b->stream>>>(view_of(b), d_ids, count, make_uint4(seed[0], seed[1], seed[2], seed[3]), signal_only,
+                                                       tail, b->model.is_float);
     if (order_leave(b, b->stream)) return -1;
     CK(cudaStreamSynchronize(b->stream));
     if (d_ids) cudaFree(d_ids);
     if (!signal_only) {
-        if (ids) for (int k = 0; k < count; k++) (*b->fc)[ids[k]] = 0;
-        else std::fill(b->fc->begin(), b->fc->end(), 0);
-        if (!ids) { b->cond_last = -1; b->deferred_fill = 0; }
+        if (ids) for (int k = 0; k < count; k++) { (*b->fc)[ids[k]] = 0; (*b->dfill)[ids[k]] = 0; }
+        else { std::fill(b->fc->begin(), b->fc->end(), 0); std::fill(b->dfill->begin(), b->dfill->end(), 0); b->deferred_fill = 0; }
     }
     return 0;
 }
@@ -306,19 +395,17 @@ LPCNetB200Batch *lpcnet_b200_batch_create_ex(int n_streams, const unsigned char 
     b->kev = new std::vector<cudaEvent_t>();
     b->fc = new std::vector<int>(n_streams, 0);
     b->deferred = new std::vector<float>();
+    b->dfill = new std::vector<int>(n_streams, 0);
     ModelConfig mc{-1.f, -1, -1};
     if (cfg) { mc.lpc_gamma = cfg->lpc_gamma; mc.features_delay = cfg->features_delay; mc.end2end = cfg->end2end; }
-    if (model_load(&b->model, blob, blob_len, &mc) != 0) { delete b->kev; delete b->fc; delete b->deferred; free(b); return nullptr; }
+    if (model_load(&b->model, blob, blob_len, &mc) != 0) { delete b->kev; delete b->fc; delete b->deferred; delete b->dfill; free(b); return nullptr; }
     const size_t n = n_streams;
     const int na = b->model.na;
-    bool ok = alloc_sample_state(&b->ss, n, na) == 0;
+    bool ok = alloc_sample_state(&b->ss, n, na) == 0 && alloc_frame_state(&b->fs, n);
     auto al = [&](void **p, size_t bytes) { if (ok && cudaMalloc(p, bytes) != cudaSuccess) ok = false; };
-    al((void **)&b->fs.conv1_state, sizeof(float) * 2 * FRAME_IN * n); al((void **)&b->fs.conv2_state, sizeof(float) * 2 * COND * n);
-    al((void **)&b->fs.lpc_carry, sizeof(float) * 2 * LPC_ORDER * n); al((void **)&b->fs.vq_mem, sizeof(float) * NB_BANDS * n);
-    al((void **)&b->fs.frame_count, sizeof(int) * n);
     al((void **)&b->fs.work, sizeof(float) * frame_work_floats(n));
-    al((void **)&b->condA, sizeof(float) * (size_t)CHUNK * condA_frame_floats(b->model.is_float != 0, n, na)); al((void **)&b->condB, sizeof(float) * (size_t)CHUNK * n * 3 * NB);
-    al((void **)&b->lpc_raw, sizeof(float) * (size_t)(CHUNK + 2) * n * LPC_ORDER);
+    al((void **)&b->condA, sizeof(float) * (size_t)(CHUNK + 1) * condA_frame_floats(b->model.is_float != 0, n, na)); al((void **)&b->condB, sizeof(float) * (size_t)(CHUNK + 1) * n * 3 * NB);
+    al((void **)&b->lpc_raw, sizeof(float) * (size_t)(CHUNK + 3) * n * LPC_ORDER);
     if (ok && cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) != cudaSuccess) ok = false;
     if (ok && (cudaStreamCreateWithFlags(&b->fs.side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&b->fs.ev_fork, cudaEventDisableTiming) != cudaSuccess ||
                cudaEventCreateWithFlags(&b->fs.ev_join, cudaEventDisableTiming) != cudaSuccess)) ok = false;
@@ -360,11 +447,11 @@ void lpcnet_b200_batch_destroy(LPCNetB200Batch *b)
     if (b->sink_ev) cudaEventDestroy(b->sink_ev);
     if (b->sink_done) cudaEventDestroy(b->sink_done);
     free_sample_state(&b->ss); free_sample_state(&b->shadow);
-    void *ptrs[] = {b->fs.conv1_state, b->fs.conv2_state, b->fs.lpc_carry, b->fs.vq_mem, b->fs.frame_count, b->fs.work, b->condA, b->condB, b->lpc_raw,
-                    b->d_features, b->d_pcm, b->d_packets, b->d_state, b->d_nsil};
+    free_frame_state(&b->fs); free_frame_state(&b->fshadow);
+    void *ptrs[] = {b->fs.work, b->condA, b->condB, b->lpc_raw, b->d_features, b->d_pcm, b->d_packets, b->d_state, b->d_nsil, b->d_keep};
     for (void *p : ptrs) if (p) cudaFree(p);
     if (b->kev) { for (cudaEvent_t e : *b->kev) cudaEventDestroy(e); delete b->kev; }
-    delete b->fc; delete b->deferred;
+    delete b->fc; delete b->deferred; delete b->dfill;
     model_free(&b->model);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
@@ -407,10 +494,8 @@ static int launch_sample(LPCNetB200Batch *b, int pos, int nf, int spf, short *pc
 #ifdef LPCNET_TRACE
     { static long long *d_trace = nullptr; if (!d_trace) { CK(cudaMalloc(&d_trace, (8 * 32 + 8 * 32 * 16) * 8)); CK(cudaMemset(d_trace, 0, (8 * 32 + 8 * 32 * 16) * 8)); } p.trace = d_trace; g_trace = d_trace; }
 #endif
-    const int d = b->model.cfg.end2end ? 0 : b->model.cfg.features_delay;   // frame f uses lpc_raw entry f + 2 - d (frame_kernels.cu)
-    p.condA = b->condA + (size_t)pos * condA_frame_floats(b->model.is_float != 0, n, na);
-    p.condB = b->condB + (size_t)pos * n * 3 * NB;
-    p.lpc_raw = b->lpc_raw + (size_t)(pos + 2 - d) * n * LPC_ORDER;
+    const CondFrame c = frame_at(b, pos);
+    p.condA = c.A; p.condB = c.B; p.lpc_raw = c.L;
     p.gamma_pow = b->model.gamma_pow;
     p.hA = b->ss.hA; p.hB = b->ss.hB; p.last_sig = b->ss.last_sig; p.deemph = b->ss.deemph; p.last_exc = b->ss.last_exc; p.rng = b->ss.rng;
     p.pcm = pcm;
@@ -590,12 +675,17 @@ int lpcnet_b200_batch_run_frame_network(LPCNetB200Batch *b, const float *feature
     return 0;
 }
 
-// lpcnet_synthesize_tail_impl (lpcnet.c:235-271): `samples` more samples with the conditioning of the last frame-network run
+// lpcnet_synthesize_tail_impl (lpcnet.c:235-271): `samples` more samples with the conditioning of the last synthesize /
+// run_frame_network call (zeros after a reset, what the snapshot held after a restore)
 int lpcnet_b200_batch_synthesize_tail(LPCNetB200Batch *b, int samples, short *pcm, int preload)
 {
     if (!b || !pcm || samples < 1 || samples > 65536) { set_error("synthesize_tail: bad arguments"); return -1; }
     if (preload < 0 || preload > samples) { set_error("preload must be in 0..samples"); return -1; }
-    if (b->cond_last < 0) { set_error("synthesize_tail: no frame network output yet"); return -1; }
+    if (b->cond_last < 0) {
+        set_error("synthesize_tail: a stream was imported since the last frame-network run and the exported state carries no conditioning; "
+                  "call synthesize or run_frame_network first");
+        return -1;
+    }
     CK(cudaSetDevice(b->device));
     const size_t pbytes = sizeof(short) * (size_t)b->n * samples;
     if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, pbytes)) return -1;
@@ -617,7 +707,8 @@ int lpcnet_b200_batch_synthesize_tail(LPCNetB200Batch *b, int samples, short *pc
 }
 
 // run_frame_network_deferred / _flush (lpcnet.c:122-144): queue up to 4 feature frames without evaluating the network; the
-// flush runs the frame network over them (outputs discarded, state and frame counters advance)
+// flush runs the frame network over each stream's queue (outputs discarded, state and frame counters advance).  As in the
+// reference, a flush leaves the conditioning a tail reads as it was.
 int lpcnet_b200_batch_frame_network_deferred(LPCNetB200Batch *b, const float *features, int feature_stride)
 {
     if (!b || !features || feature_stride < NB_FEAT) { set_error("frame_network_deferred: bad arguments"); return -1; }
@@ -626,6 +717,7 @@ int lpcnet_b200_batch_frame_network_deferred(LPCNetB200Batch *b, const float *fe
     float *q = b->deferred->data();
     if (b->deferred_fill == DEFER_MAX) memmove(q, q + fr, sizeof(float) * fr * (DEFER_MAX - 1));
     else b->deferred_fill++;
+    for (int &v : *b->dfill) v = std::min(DEFER_MAX, v + 1);
     float *dst = q + fr * (b->deferred_fill - 1);
     for (int s = 0; s < b->n; s++) memcpy(dst + (size_t)s * NB_FEAT, features + (size_t)s * feature_stride, sizeof(float) * NB_FEAT);
     return 0;
@@ -633,14 +725,44 @@ int lpcnet_b200_batch_frame_network_deferred(LPCNetB200Batch *b, const float *fe
 int lpcnet_b200_batch_frame_network_flush(LPCNetB200Batch *b)
 {
     if (!b) { set_error("null batch"); return -1; }
-    const int fill = b->deferred_fill;
-    if (fill == 0) return 0;
-    const size_t fr = (size_t)b->n * NB_FEAT;
-    std::vector<float> f((size_t)b->n * fill * NB_FEAT);             // [n][fill][20]
-    for (int k = 0; k < fill; k++) for (int s = 0; s < b->n; s++)
-        memcpy(&f[((size_t)s * fill + k) * NB_FEAT], b->deferred->data() + fr * k + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
+    const int F = b->deferred_fill, n = b->n;
+    const std::vector<int> fill = *b->dfill;
     b->deferred_fill = 0;
-    return lpcnet_b200_batch_run_frame_network(b, f.data(), fill, NB_FEAT);
+    std::fill(b->dfill->begin(), b->dfill->end(), 0);
+    // stream s runs queued frame k iff k >= F - fill[s]; from frame k_all on every stream does
+    int k0 = F, k_all = 0;
+    for (int v : fill) { k0 = std::min(k0, F - v); k_all = std::max(k_all, F - v); }
+    if (k0 >= F) return 0;
+    CK(cudaSetDevice(b->device));
+    const size_t fr = (size_t)n * NB_FEAT;
+    std::vector<float> f((size_t)n * F * NB_FEAT);                   // [n][F][20]
+    std::vector<int> keep((size_t)F * n);                            // [F][n]
+    for (int k = 0; k < F; k++) for (int s = 0; s < n; s++) {
+        memcpy(&f[((size_t)s * F + k) * NB_FEAT], b->deferred->data() + fr * k + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
+        keep[(size_t)k * n + s] = k < F - fill[s];
+    }
+    if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * f.size())) return -1;
+    if (k_all > k0) {
+        if (!b->fshadow.conv1_state && !alloc_frame_state(&b->fshadow, n)) { set_error("flush: device allocation failed"); return -1; }
+        if (!b->d_keep) CK(cudaMalloc((void **)&b->d_keep, sizeof(int) * DEFER_MAX * n));
+    }
+    cudaStream_t st = b->stream;
+    if (order_enter(b, st)) return -1;
+    CK(cudaMemcpyAsync(b->d_features, f.data(), sizeof(float) * f.size(), cudaMemcpyHostToDevice, st));
+    if (k_all > k0) CK(cudaMemcpyAsync(b->d_keep, keep.data(), sizeof(int) * keep.size(), cudaMemcpyHostToDevice, st));
+    if (park_tail(b, st)) return -1;
+    for (int k = k0; k < k_all; k++) {       // frames only some streams run: one launch per frame, the others' 100 Hz state put back after it
+        if (copy_frame_state(b->fshadow, b->fs, n, st)) return -1;
+        launch_frame_network(b->model, b->fs, b->d_features + (size_t)k * NB_FEAT, (long long)F * NB_FEAT, NB_FEAT, n, 1, b->condA, b->condB, b->lpc_raw, st);
+        keep_frame_state_kernel<<<n, 128, 0, st>>>(b->fs, b->fshadow, b->d_keep + (size_t)k * n, n);
+    }
+    if (k_all < F)
+        launch_frame_network(b->model, b->fs, b->d_features + (size_t)k_all * NB_FEAT, (long long)F * NB_FEAT, NB_FEAT, n, F - k_all, b->condA, b->condB, b->lpc_raw, st);
+    CK(cudaGetLastError());
+    for (int s = 0; s < n; s++) (*b->fc)[s] = std::min(1000, (*b->fc)[s] + fill[s]);
+    if (order_leave(b, st)) return -1;
+    CK(cudaStreamSynchronize(st));                                   // (f and keep are read by the copies above)
+    return 0;
 }
 
 static int decode_device(LPCNetB200Batch *b, const uint8_t *d_packets, int npackets, short *d_pcm, cudaStream_t st)
@@ -819,6 +941,10 @@ int lpcnet_b200_batch_state_size(const LPCNetB200Batch *b)
 static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
 {
     if (!b || !buf || s < 0 || s >= b->n) { set_error("state export/import: bad arguments"); return -1; }
+    if (!dir && (*b->dfill)[s] > 0) {
+        set_error("export_state: stream %d has %d queued frames and the exported state has no room for them; flush first", s, (*b->dfill)[s]);
+        return -1;
+    }
     CK(cudaSetDevice(b->device));
     const size_t bytes = (size_t)state_words(b->model.na) * 4;
     if (ensure(b, (void **)&b->d_state, &b->d_state_cap, bytes)) return -1;
@@ -831,6 +957,8 @@ static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
     if (dir) {
         int fcv; memcpy(&fcv, (const char *)buf + (size_t)(state_words(b->model.na) - 5) * 4, 4);
         (*b->fc)[s] = fcv;
+        (*b->dfill)[s] = 0;
+        b->cond_last = -1;          // the blob carries no conditioning: no tail until the next frame-network run
     }
     return 0;
 }
@@ -838,19 +966,21 @@ int lpcnet_b200_batch_export_state(LPCNetB200Batch *b, int s, void *buf) { retur
 int lpcnet_b200_batch_import_state(LPCNetB200Batch *b, int s, const void *buf) { return state_move(b, s, const_cast<void *>(buf), 1); }
 
 // ---- whole-batch snapshot on the device (roll-back after speculative synthesis) ----
+// It also holds the frame a tail reads, as the reference's state copy holds gru_a_condition / gru_b_condition / lpc.
 struct LPCNetB200Snapshot {
-    int n, na, device;
-    SampleState ss; FrameState fs;
-    std::vector<int> *fc; int cond_last; int deferred_fill; std::vector<float> *deferred;
+    int n, na, device; size_t fa;
+    SampleState ss; FrameState fs; CondFrame tail;
+    std::vector<int> *fc; int cond_last; int deferred_fill; std::vector<float> *deferred; std::vector<int> *dfill;
 };
 void lpcnet_b200_batch_snapshot_destroy(LPCNetB200Snapshot *s)
 {
     if (!s) return;
     cudaSetDevice(s->device);
     free_sample_state(&s->ss);
-    void *ptrs[] = {s->fs.conv1_state, s->fs.conv2_state, s->fs.lpc_carry, s->fs.vq_mem, s->fs.frame_count};
+    free_frame_state(&s->fs);
+    void *ptrs[] = {s->tail.A, s->tail.B, s->tail.L};
     for (void *p : ptrs) if (p) cudaFree(p);
-    delete s->fc; delete s->deferred;
+    delete s->fc; delete s->deferred; delete s->dfill;
     free(s);
 }
 LPCNetB200Snapshot *lpcnet_b200_batch_snapshot_create(LPCNetB200Batch *b)
@@ -858,45 +988,42 @@ LPCNetB200Snapshot *lpcnet_b200_batch_snapshot_create(LPCNetB200Batch *b)
     if (!b) { set_error("null batch"); return nullptr; }
     if (cudaSetDevice(b->device) != cudaSuccess) return nullptr;
     LPCNetB200Snapshot *s = (LPCNetB200Snapshot *)calloc(1, sizeof(*s));
-    s->n = b->n; s->na = b->model.na; s->device = b->device;
-    s->fc = new std::vector<int>(b->n, 0); s->deferred = new std::vector<float>();
+    s->n = b->n; s->na = b->model.na; s->device = b->device; s->fa = condA_floats(b);
+    s->fc = new std::vector<int>(b->n, 0); s->deferred = new std::vector<float>(); s->dfill = new std::vector<int>(b->n, 0);
     const size_t n = b->n;
-    bool ok = alloc_sample_state(&s->ss, n, s->na) == 0;
+    bool ok = alloc_sample_state(&s->ss, n, s->na) == 0 && alloc_frame_state(&s->fs, n);
     auto al = [&](void **p, size_t bytes) { if (ok && cudaMalloc(p, bytes) != cudaSuccess) ok = false; };
-    al((void **)&s->fs.conv1_state, sizeof(float) * 2 * FRAME_IN * n); al((void **)&s->fs.conv2_state, sizeof(float) * 2 * COND * n);
-    al((void **)&s->fs.lpc_carry, sizeof(float) * 2 * LPC_ORDER * n); al((void **)&s->fs.vq_mem, sizeof(float) * NB_BANDS * n);
-    al((void **)&s->fs.frame_count, sizeof(int) * n);
+    al((void **)&s->tail.A, sizeof(float) * s->fa); al((void **)&s->tail.B, sizeof(float) * n * 3 * NB); al((void **)&s->tail.L, sizeof(float) * n * LPC_ORDER);
     if (!ok) { set_error("snapshot: device allocation failed"); lpcnet_b200_batch_snapshot_destroy(s); return nullptr; }
     return s;
 }
-static int copy_frame_state(const FrameState &dst, const FrameState &src, size_t n, cudaStream_t st)
+static bool snapshot_fits(const LPCNetB200Batch *b, const LPCNetB200Snapshot *s)
 {
-    CK(cudaMemcpyAsync(dst.conv1_state, src.conv1_state, sizeof(float) * 2 * FRAME_IN * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.conv2_state, src.conv2_state, sizeof(float) * 2 * COND * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.lpc_carry, src.lpc_carry, sizeof(float) * 2 * LPC_ORDER * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.vq_mem, src.vq_mem, sizeof(float) * NB_BANDS * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.frame_count, src.frame_count, sizeof(int) * n, cudaMemcpyDeviceToDevice, st));
-    return 0;
+    if (b && s && s->n == b->n && s->na == b->model.na && s->device == b->device && s->fa == condA_floats(b)) return true;
+    set_error("snapshot does not belong to this batch");
+    return false;
 }
 int lpcnet_b200_batch_snapshot_save(LPCNetB200Batch *b, LPCNetB200Snapshot *s)
 {
-    if (!b || !s || s->n != b->n || s->na != b->model.na || s->device != b->device) { set_error("snapshot does not belong to this batch"); return -1; }
+    if (!snapshot_fits(b, s)) return -1;
     CK(cudaSetDevice(b->device));
     if (order_enter(b, b->stream)) return -1;
     if (copy_sample_state(s->ss, b->ss, b->n, s->na, b->stream) || copy_frame_state(s->fs, b->fs, b->n, b->stream)) return -1;
+    if (b->cond_last >= 0 && copy_cond_frame(b, s->tail, frame_at(b, b->cond_last), b->stream)) return -1;
     if (order_leave(b, b->stream)) return -1;
-    *s->fc = *b->fc; s->cond_last = b->cond_last; s->deferred_fill = b->deferred_fill; *s->deferred = *b->deferred;
+    *s->fc = *b->fc; s->cond_last = b->cond_last; s->deferred_fill = b->deferred_fill; *s->deferred = *b->deferred; *s->dfill = *b->dfill;
     return 0;
 }
 int lpcnet_b200_batch_snapshot_restore(LPCNetB200Batch *b, const LPCNetB200Snapshot *s)
 {
-    if (!b || !s || s->n != b->n || s->na != b->model.na || s->device != b->device) { set_error("snapshot does not belong to this batch"); return -1; }
+    if (!snapshot_fits(b, s)) return -1;
     CK(cudaSetDevice(b->device));
     if (order_enter(b, b->stream)) return -1;
     if (copy_sample_state(b->ss, s->ss, b->n, s->na, b->stream) || copy_frame_state(b->fs, s->fs, b->n, b->stream)) return -1;
+    if (s->cond_last >= 0 && copy_cond_frame(b, frame_at(b, TAIL_SLOT), s->tail, b->stream)) return -1;
     if (order_leave(b, b->stream)) return -1;
-    *b->fc = *s->fc; b->deferred_fill = s->deferred_fill; *b->deferred = *s->deferred;
-    b->cond_last = -1;            // the conditioning buffers are not part of the snapshot: a tail call needs a fresh frame-network run
+    *b->fc = *s->fc; b->deferred_fill = s->deferred_fill; *b->deferred = *s->deferred; *b->dfill = *s->dfill;
+    b->cond_last = s->cond_last >= 0 ? TAIL_SLOT : -1;
     return 0;
 }
 

@@ -432,6 +432,7 @@ VARIANTS = {
     "e2e":    dict(e2e=True, delay=2, gamma=1.0),         # END2END: LPC from the network's reflection coefficients (lpcnet.c:57-78,107-108)
     "delay0": dict(delay=0),                              # FEATURES_DELAY 0: no look-ahead, LPC of the current frame (lpcnet.c:113-115)
     "na256e2e": dict(na=256, e2e=True, delay=0, gamma=0.95),
+    "delay1": dict(delay=1),                              # FEATURES_DELAY 1: a one-frame LPC delay line (lpcnet.c:109-112)
 }
 
 

@@ -452,12 +452,12 @@ int oracle_pitch_index(float f)
     return pitch > 255 ? 255 : (pitch < 33 ? 33 : pitch);          /* IMIN(255, IMAX(33, pitch)) */
 }
 
-static void run_frame_network(OState *st, const float *features)     /* lpcnet.c:82-120 */
+/* lpcnet.c:82-120: the conditioning and the weighted LPC go to gru_a / gru_b / lpc (the state's own arrays, or a flush's locals) */
+static void run_frame_network(OState *st, float *gru_a, float *gru_b, float *lpc, const float *features)
 {
     const OModel *m = st->m;
     const int N_A = m->na, delay = m->features_delay;
     float in[FRAME_IN], conv1_out[COND], conv2_out[COND], dense1_out[COND], condition[COND];
-    float *lpc = st->lpc;
     int pitch = oracle_pitch_index(features[NB_BANDS]), i;
     memcpy(in, features, sizeof(float) * NB_FEATURES);
     memcpy(in + NB_FEATURES, m->embed_pitch + pitch * PITCH_EMBED, sizeof(float) * PITCH_EMBED);
@@ -467,8 +467,8 @@ static void run_frame_network(OState *st, const float *features)     /* lpcnet.c
     if (st->frame_count < delay) memset(conv2_out, 0, sizeof(conv2_out));
     dense(m, dense1_out, m->dense1_w, m->dense1_b, COND, COND, conv2_out, 1);
     dense(m, condition, m->dense2_w, m->dense2_b, COND, COND, dense1_out, 1);
-    dense(m, st->gru_a_condition, m->gad_w, m->gad_b, COND, 3 * N_A, condition, 0);
-    dense(m, st->gru_b_condition, m->gbd_w, m->gbd_b, COND, 3 * N_B, condition, 0);
+    dense(m, gru_a, m->gad_w, m->gad_b, COND, 3 * N_A, condition, 0);
+    dense(m, gru_b, m->gbd_w, m->gbd_b, COND, 3 * N_B, condition, 0);
     if (m->end2end) rc2lpc(lpc, condition);                        /* lpcnet.c:105,107-108 */
     else if (delay > 0) {                                          /* lpcnet.c:109-112 */
         memcpy(lpc, st->old_lpc[delay - 1], sizeof(float) * LPC_ORDER);
@@ -718,7 +718,7 @@ void oracle_state_destroy(OState *st) { free(st); }
 
 void oracle_synthesize_impl(OState *st, const float *features, short *output, int N, int preload)   /* lpcnet_synthesize_impl lpcnet.c:273-277 */
 {
-    run_frame_network(st, features);
+    run_frame_network(st, st->gru_a_condition, st->gru_b_condition, st->lpc, features);
     synthesize_tail(st, output, N, preload);
 }
 void oracle_synthesize(OState *st, const float *features, short *output, int N)   /* lpcnet_synthesize lpcnet.c:279-281 */
@@ -726,7 +726,7 @@ void oracle_synthesize(OState *st, const float *features, short *output, int N) 
     oracle_synthesize_impl(st, features, output, N, 0);
 }
 /* the other internal entry points the PLC uses (lpcnet_private.h:125-133) */
-void oracle_run_frame_network(OState *st, const float *features) { run_frame_network(st, features); }
+void oracle_run_frame_network(OState *st, const float *features) { run_frame_network(st, st->gru_a_condition, st->gru_b_condition, st->lpc, features); }
 void oracle_synthesize_tail(OState *st, short *output, int N, int preload) { synthesize_tail(st, output, N, preload); }
 void oracle_frame_network_deferred(OState *st, const float *features)             /* run_frame_network_deferred lpcnet.c:122-132 */
 {
@@ -738,7 +738,10 @@ void oracle_frame_network_deferred(OState *st, const float *features)           
 void oracle_frame_network_flush(OState *st)                                       /* run_frame_network_flush lpcnet.c:134-144 */
 {
     int i;
-    for (i = 0; i < st->feature_buffer_fill; i++) run_frame_network(st, &st->feature_buffer[i * NB_FEATURES]);
+    for (i = 0; i < st->feature_buffer_fill; i++) {
+        float gru_a[3 * N_A_MAX], gru_b[3 * N_B], lpc[LPC_ORDER];         /* locals: a later tail still reads the last synthesize / run_frame_network */
+        run_frame_network(st, gru_a, gru_b, lpc, &st->feature_buffer[i * NB_FEATURES]);
+    }
     st->feature_buffer_fill = 0;
 }
 void oracle_reset_signal(OState *st)                                              /* lpcnet_reset_signal lpcnet.c:226-233 */
@@ -782,7 +785,7 @@ void oracle_decode_packet(OState *st, float *features /*[4][36]*/, const unsigne
 /* taps for unit tests */
 void oracle_frame_network(OState *st, const float *features, float *ga /*1152*/, float *gb /*48*/, float *lpc /*16*/)
 {
-    run_frame_network(st, features);
+    run_frame_network(st, st->gru_a_condition, st->gru_b_condition, st->lpc, features);
     memcpy(ga, st->gru_a_condition, sizeof(float) * 3 * st->m->na);
     memcpy(gb, st->gru_b_condition, sizeof(st->gru_b_condition));
     memcpy(lpc, st->lpc, sizeof(st->lpc));

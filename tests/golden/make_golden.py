@@ -42,7 +42,7 @@ print(json.dumps(dig, indent=1))
 # ---- model variants (SURVEY 8f N1): the reference compiled with each variant's generated nnet_data.h (oracle/Makefile VARIANTS)
 var = {}
 fv = make_feature_batch(range(2), 20)
-for tag in ("na256", "na128", "e2e", "delay0", "na256e2e"):
+for tag in ("na256", "na128", "e2e", "delay0", "na256e2e", "delay1"):
     for build in ("A", "B"):
         var["%s_%s" % (tag, build)] = H.ref_synth(fv, build, tag=tag)
 np.savez_compressed(os.path.join(HERE, "variants.npz"), **var)

@@ -15,9 +15,10 @@ def plc_like_script(T):
     s += [("net", 6), ("tail", 80, 0), ("tail", 80, 0)]           # run_frame_network + two half-frame tails (PLC uses N=80)
     s += [("net", 7), ("tail", 160, 160)]                         # a fully teacher-forced frame (state update only)
     s += [("defer", 8), ("defer", 9), ("flush",)]                 # queued conditioning frames, network run later
-    s += [("synth", 10, 160, 0), ("reset_signal",), ("synth", 11, 160, 0)]
-    s += [("save",), ("synth", 12, 160, 0), ("synth", 13, 160, 0), ("restore",), ("synth", 12, 160, 0), ("synth", 13, 160, 0)]
-    s += [("synth", t, 160, 0) for t in range(14, T)]
+    s += [("net", 10), ("defer", 11), ("defer", 12), ("flush",), ("tail", 80, 0)]    # a flush keeps the conditioning a tail reads (lpcnet.c:134-144)
+    s += [("synth", 13, 160, 0), ("reset_signal",), ("synth", 14, 160, 0)]
+    s += [("save",), ("synth", 15, 160, 0), ("synth", 16, 160, 0), ("restore",), ("synth", 15, 160, 0), ("synth", 16, 160, 0)]
+    s += [("synth", t, 160, 0) for t in range(17, T)]
     return s
 
 
@@ -73,6 +74,10 @@ class RefState:
         c = self(); self.L.ref_state_copy(c, st); return c
     def assign(self, dst, src):
         self.L.ref_state_copy(dst, src)
+    def reset(self, st):
+        self.L.ref_state_reset(st)
+    def destroy(self, st):
+        self.L.ref_state_destroy(st)
 
 
 class OracleState:
@@ -85,6 +90,10 @@ class OracleState:
         c = self(); ctypes.memmove(c, st, self.L.oracle_state_size()); return c
     def assign(self, dst, src):
         ctypes.memmove(dst, src, self.L.oracle_state_size())
+    def reset(self, st):
+        self.L.oracle_reset(st)
+    def destroy(self, st):
+        self.L.oracle_state_destroy(st)
 
 
 def run_engine(batch, feats, streams, script):
@@ -111,6 +120,291 @@ def run_engine(batch, feats, streams, script):
             snap = batch.snapshot()
         elif op[0] == "restore":
             batch.restore(snap)
+    if snap is not None:
+        batch.free_snapshot(snap)
+    return np.concatenate(out, axis=1)
+
+
+# ---- random call sequences over a batch of streams ------------------------------------------------------------------------------
+# A script is (ops, T, signal): batch operations over feature frames 0..T-1 and the kind of signal the teacher-forced samples come from.
+#   ("synth", t, k, N, pre)   frames t..t+k-1, N samples each, `pre` forced samples at the start of the first frame
+#   ("net", t, k)             run_frame_network over frames t..t+k-1
+#   ("tail", N, pre)          synthesize_tail
+#   ("defer", t)              run_frame_network_deferred of frame t
+#   ("flush",) ("reset_signal",) ("reset",) ("save",) ("restore",)
+#   ("reset_streams", ids)    lpcnet_reset of the listed streams
+#   ("move", a, b)            export stream a, import the blob into stream b
+# Only what the batched ABI allows is generated: stream a of a move has no queued frames, and no tail follows a move before
+# the next synth / net (the exported state carries neither the queue nor the conditioning).
+OUTPUT_OPS = ("synth", "tail")
+SYNTH_FRAMES = (1, 2, 3, 17, 20)            # 17 and 20 cross the engine's 16-frame chunk
+SAMPLES = (1, 80, 160, 250)
+
+
+def _preload(rng, N):
+    r = rng.random()
+    return 0 if r < 0.5 else (N if r < 0.75 else rng.randint(1, min(N, 40)))
+
+
+def random_script(seed, n_streams, n_ops=22):
+    import random
+    rng = random.Random(seed)
+    ops, t = [], 0
+    fill = [0] * n_streams               # queued frames per stream
+    no_tail = False                       # a move since the last synth / net
+    saved = None                          # (fill, no_tail) at the last save
+    signal = rng.choice(["speech", "square"])
+
+    def synth():
+        nonlocal t, no_tail
+        k = rng.choice(SYNTH_FRAMES) if rng.random() < 0.35 else rng.choice((1, 1, 2, 3))
+        N = rng.choice(SAMPLES)
+        ops.append(("synth", t, k, N, _preload(rng, N))); t += k; no_tail = False
+
+    def tail():
+        if not no_tail:
+            N = rng.choice(SAMPLES)
+            ops.append(("tail", N, _preload(rng, N)))
+
+    def flush():
+        ops.append(("flush",))
+        fill[:] = [0] * n_streams
+
+    def reset_streams():
+        ids = sorted(rng.sample(range(n_streams), rng.randint(1, max(1, n_streams // 2))))
+        if rng.random() < 0.5:
+            ids = sorted(set(ids) | {rng.choice((0, n_streams - 1))})
+        ops.append(("reset_streams", ids))
+        for s in ids:
+            fill[s] = 0
+
+    synth()
+    while len(ops) < n_ops:
+        op = rng.choices(["synth", "net", "tail", "defer", "flush", "reset_signal", "reset", "reset_streams", "save", "restore", "move"],
+                         [5, 2, 2, 3, 2, 1, 1, 2, 1, 1, 1])[0]
+        if op == "synth":
+            synth()
+        elif op == "net":
+            k = rng.choice((1, 2, 3))
+            ops.append(("net", t, k)); t += k; no_tail = False
+            if rng.random() < 0.5:
+                tail()
+        elif op == "tail":
+            tail()
+        elif op == "defer":
+            for _ in range(rng.choice((1, 2, 3, 5, 6))):          # 5-6: the oldest queued frames drop out
+                ops.append(("defer", t)); t += 1
+                fill[:] = [min(4, v + 1) for v in fill]
+            r = rng.random()
+            if r < 0.3:
+                reset_streams()                                   # with queued frames: only the other streams' queues stay
+            if r < 0.7:
+                flush()
+                if rng.random() < 0.7:
+                    tail()
+        elif op == "flush":
+            flush()
+        elif op == "reset_signal":
+            ops.append(("reset_signal",))
+        elif op == "reset":
+            ops.append(("reset",)); fill[:] = [0] * n_streams; no_tail = False
+            if rng.random() < 0.5:
+                tail()
+        elif op == "reset_streams":
+            reset_streams()
+            r = rng.random()
+            if r < 0.4:
+                synth()                                           # within FEATURES_DELAY frames of the reset: a mixed silent segment
+            elif r < 0.7 and any(fill):
+                flush()
+                tail()
+        elif op == "save":
+            ops.append(("save",)); saved = (list(fill), no_tail)
+        elif op == "restore" and saved is not None:
+            ops.append(("restore",)); fill[:] = saved[0]; no_tail = saved[1]
+            if rng.random() < 0.6:
+                tail()
+        elif op == "move":
+            ok = [s for s in range(n_streams) if fill[s] == 0]
+            if ok:
+                a = rng.choice(ok)
+                b = rng.choice([s for s in range(n_streams) if s != a] or [a])
+                ops.append(("move", a, b)); fill[b] = 0; no_tail = True
+    return ops, t, signal
+
+
+def script_events(script, n_streams, delay=2):
+    """The situations a script reaches, found by following each stream's queue and frame counter: a set of names."""
+    ev = set()
+    fill, fc = [0] * n_streams, [0] * n_streams
+    prev, saved = None, None
+    for op in script[0]:
+        kind = tag = op[0]
+        ev.add(kind)
+        if kind == "synth":
+            k, N, pre = op[2:]
+            if pre == N and k > 1:
+                ev.add("preload_N_multi_frame")
+            if k > 16:
+                ev.add("synth_crosses_chunk")
+            if min(k, max(0, delay - min(fc))) > min(k, max(0, delay - max(fc))):     # some streams silent, others not
+                ev.add("mixed_silent_segment")
+            fc = [min(1000, v + k) for v in fc]
+        elif kind == "net":
+            fc = [min(1000, v + op[2]) for v in fc]
+        elif kind == "defer":
+            if 4 in fill:
+                ev.add("queue_overflow")
+            fill = [min(4, v + 1) for v in fill]
+        elif kind == "flush":
+            if any(fill):
+                tag = "flush+"
+                if prev == "reset_streams+":
+                    ev.add("flush_after_reset_streams_with_queue")
+                if len(set(fill)) > 1:
+                    ev.add("flush_uneven_queues")
+            fc = [min(1000, v + f) for v, f in zip(fc, fill)]
+            fill = [0] * n_streams
+        elif kind == "tail":
+            ev.add({"flush+": "tail_after_nonempty_flush", "reset": "tail_after_reset", "restore": "tail_after_restore"}.get(prev, "tail"))
+        elif kind == "reset":
+            fill, fc = [0] * n_streams, [0] * n_streams
+        elif kind == "reset_streams":
+            if any(fill[s] for s in op[1]):
+                tag = "reset_streams+"
+            if 0 in op[1] or n_streams - 1 in op[1]:
+                ev.add("reset_streams_edge")
+            for s in op[1]:
+                fill[s] = fc[s] = 0
+        elif kind == "save":
+            saved = (list(fill), list(fc))
+        elif kind == "restore":
+            fill, fc = list(saved[0]), list(saved[1])
+        elif kind == "move":
+            fc[op[2]] = fc[op[1]]
+            fill[op[2]] = 0
+        prev = tag
+    return ev
+
+
+def script_outputs(script):
+    """Samples per stream the script's synth and tail ops produce."""
+    return sum(op[2] * op[3] if op[0] == "synth" else op[1] for op in script[0] if op[0] in OUTPUT_OPS)
+
+
+def forced_pcm(signal, stream, n):
+    """Teacher-forcing signal of one stream: the speech-like forced_signal, or a full-scale square wave (+32767 / -32768) that
+    drives lin2ulaw of the forced excitation to its clamps."""
+    if signal == "square":
+        period = 24 + 2 * (int(stream) % 7)
+        return np.where(np.arange(n) % period < period // 2, 32767, -32768).astype(np.int16)
+    rng = np.random.default_rng(5000 + int(stream))
+    return (3000 * np.sin(np.arange(n) * 0.05 * (1 + stream % 3)) + rng.normal(0, 300, n)).astype(np.int16)
+
+
+def run_streams(backend, lib, factory, feats, streams, script, pool=None):
+    """A script on one single-stream state per stream (backend 'ref' | 'oracle').  feats [n][T][20].  reset_streams resets the
+    listed states, a move copies the whole source state, a snapshot copies every state.  Returns PCM [n][script_outputs]."""
+    ops, _, signal = script
+    n = len(streams)
+    P = (dict(impl=lib.ref_synthesize_impl, net=lib.ref_run_frame_network, tail=lib.ref_synthesize_tail, defer=lib.ref_frame_network_deferred,
+              flush=lib.ref_frame_network_flush, rs=lib.ref_reset_signal) if backend == "ref" else
+         dict(impl=lib.oracle_synthesize_impl, net=lib.oracle_run_frame_network, tail=lib.oracle_synthesize_tail, defer=lib.oracle_frame_network_deferred,
+              flush=lib.oracle_frame_network_flush, rs=lib.oracle_reset_signal))
+    total = script_outputs(script)
+    forced = [forced_pcm(signal, s, total) for s in streams]
+    out = np.zeros((n, total), np.int16)
+    st = [factory() for _ in range(n)]
+    snap = None
+    k = 0
+
+    def each(fn):
+        list(pool.map(fn, range(n))) if pool is not None else [fn(i) for i in range(n)]
+
+    for op in ops:
+        kind = op[0]
+        if kind == "synth":
+            _, t, nf, N, pre = op
+            def run(i, t=t, nf=nf, N=N, pre=pre, k=k):
+                for j in range(nf):
+                    buf = out[i, k + j * N:k + (j + 1) * N]
+                    if j == 0:
+                        buf[:pre] = forced[i][k:k + pre]
+                    P["impl"](st[i], feats[i, t + j].ctypes.data, buf.ctypes.data, N, pre if j == 0 else 0)
+            each(run); k += nf * N
+        elif kind == "net":
+            _, t, nf = op
+            each(lambda i: [P["net"](st[i], feats[i, t + j].ctypes.data) for j in range(nf)])
+        elif kind == "tail":
+            _, N, pre = op
+            def run(i, N=N, pre=pre, k=k):
+                buf = out[i, k:k + N]
+                buf[:pre] = forced[i][k:k + pre]
+                P["tail"](st[i], buf.ctypes.data, N, pre)
+            each(run); k += N
+        elif kind == "defer":
+            for i in range(n):
+                P["defer"](st[i], feats[i, op[1]].ctypes.data)
+        elif kind == "flush":
+            each(lambda i: P["flush"](st[i]))
+        elif kind == "reset_signal":
+            for i in range(n):
+                P["rs"](st[i])
+        elif kind == "reset":
+            for i in range(n):
+                factory.reset(st[i])
+        elif kind == "reset_streams":
+            for i in op[1]:
+                factory.reset(st[i])
+        elif kind == "save":
+            if snap is not None:
+                for c in snap:
+                    factory.destroy(c)
+            snap = [factory.copy_of(x) for x in st]
+        elif kind == "restore":
+            for x, c in zip(st, snap):
+                factory.assign(x, c)
+        elif kind == "move":
+            factory.assign(st[op[2]], st[op[1]])
+    for x in st + (snap or []):
+        factory.destroy(x)
+    return out
+
+
+def run_engine_script(batch, feats, streams, script):
+    """The same script on a lpcnet_b200.Batch of len(streams) streams.  Returns PCM [n][script_outputs]."""
+    ops, _, signal = script
+    total = script_outputs(script)
+    forced = np.stack([forced_pcm(signal, s, total) for s in streams])
+    out, k, snap = [], 0, None
+    for op in ops:
+        kind = op[0]
+        if kind == "synth":
+            _, t, nf, N, pre = op
+            out.append(batch.synthesize(feats[:, t:t + nf], samples_per_frame=N, preload=pre, pcm_in=forced[:, k:k + max(pre, 1)])); k += nf * N
+        elif kind == "net":
+            batch.run_frame_network(feats[:, op[1]:op[1] + op[2]])
+        elif kind == "tail":
+            _, N, pre = op
+            out.append(batch.synthesize_tail(N, preload=pre, pcm_in=forced[:, k:k + max(pre, 1)])); k += N
+        elif kind == "defer":
+            batch.frame_network_deferred(feats[:, op[1]])
+        elif kind == "flush":
+            batch.frame_network_flush()
+        elif kind == "reset_signal":
+            batch.reset_signal()
+        elif kind == "reset":
+            batch.reset()
+        elif kind == "reset_streams":
+            batch.reset_streams(op[1])
+        elif kind == "save":
+            if snap is not None:
+                batch.free_snapshot(snap)
+            snap = batch.snapshot()
+        elif kind == "restore":
+            batch.restore(snap)
+        elif kind == "move":
+            batch.import_state(op[2], batch.export_state(op[1]))
     if snap is not None:
         batch.free_snapshot(snap)
     return np.concatenate(out, axis=1)

@@ -20,7 +20,7 @@ def eng():
     return lpcnet_b200
 
 
-@pytest.mark.parametrize("kind,tag,n", [("int8", "", 40), ("int8", "", 5), ("float", "", 6), ("float", "", 40), ("int8", "na256e2e", 7), ("int8", "delay0", 3)])
+@pytest.mark.parametrize("kind,tag,n", [("int8", "", 40), ("int8", "", 5), ("float", "", 6), ("float", "", 40), ("int8", "na256e2e", 7), ("int8", "delay0", 3), ("int8", "delay1", 4)])
 def test_plc_like_call_sequence_matches_oracle(eng, kind, tag, n):
     """The scripted sequence of scenarios.plc_like_script (preload, tails of 80, a fully forced frame, deferred + flush,
     reset_signal, snapshot / restore) on a batch == the same sequence per stream on the CPU restatement (which the CPU suite

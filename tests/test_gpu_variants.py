@@ -9,7 +9,7 @@ import helpers as H
 from fixtures import make_feature_batch
 
 pytestmark = pytest.mark.gpu
-TAGS = ["na256", "na128", "e2e", "delay0", "na256e2e"]
+TAGS = ["na256", "na128", "e2e", "delay0", "na256e2e", "delay1"]
 
 
 @pytest.fixture(scope="module")

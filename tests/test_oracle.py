@@ -193,7 +193,7 @@ def test_oracle_port_clamp_fixture():
     np.testing.assert_array_equal(pcm, gold)
 
 
-VARIANT_TAGS = ["na256", "na128", "e2e", "delay0", "na256e2e"]
+VARIANT_TAGS = ["na256", "na128", "e2e", "delay0", "na256e2e", "delay1"]
 
 
 @pytest.mark.parametrize("tag", VARIANT_TAGS)
@@ -212,7 +212,7 @@ def test_oracle_port_model_variants_match_reference_golden(tag, build):
 
 
 @pytest.mark.ref
-@pytest.mark.parametrize("build,tag", [("A", ""), ("B", ""), ("A", "na256e2e"), ("A", "delay0")])
+@pytest.mark.parametrize("build,tag", [("A", ""), ("B", ""), ("A", "na256e2e"), ("A", "delay0"), ("A", "delay1"), ("B", "delay1")])
 def test_oracle_port_plc_entry_points_match_reference(build, tag):
     """lpcnet_synthesize_impl(preload), run_frame_network + lpcnet_synthesize_tail_impl, deferred/flush, lpcnet_reset_signal and
     state copies (what src/lpcnet_plc.c does around the hot path): the CPU restatement against the compiled reference."""
