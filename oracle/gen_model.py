@@ -30,6 +30,7 @@ Outputs (into --out, default oracle/_gen):
                    reference is built with -DUSE_WEIGHTS_FILE and fed the blob)
 """
 import argparse
+import functools
 import os
 import struct
 import numpy as np
@@ -436,11 +437,11 @@ VARIANTS = {
 }
 
 
-def _grub_split(rng):
+def _grub_split(rng, na=N_A):
     """--grub-density 0.5 with --grub-density-split (training_tf2/train_lpcnet.py:46-78, SparsifyGRUB): the update and reset
     rows sparse with unequal counts per row group, the candidate rows dense.  Row group 0 keeps one block (the second int8 K
     part is empty), row group 2 three (a partial quad)."""
-    nin = N_A // 4
+    nin = na // 4
     keep = np.ones((nin, 6), bool)
     for rg, d in enumerate((0.15, 0.35, 0.20, 0.30)):
         keep[:, rg] = rng.random(nin) < d
@@ -450,23 +451,29 @@ def _grub_split(rng):
     return keep
 
 
-def _grub_even(rng):
-    """Every GRU_B row group keeps 42 column blocks at scattered positions: all lists alike but not dense; the int8 K parts
-    take 21 blocks each (5 full quads and a partial one)."""
-    keep = np.zeros((N_A // 4, 6), bool)
+GRUB_EVEN_BLOCKS = {384: 42, 256: 42, 128: 22}     # fewer than na/4 column blocks; each int8 K part (n/2) ends in a partial quad
+
+
+def _grub_even(rng, na=N_A):
+    """Every GRU_B row group keeps GRUB_EVEN_BLOCKS[na] column blocks at scattered positions: all lists alike but not dense; the
+    int8 K parts take half of them each (at 384 and 256: 21 blocks, 5 full quads and a partial one; at 128: 11, 2 and a partial)."""
+    nin = na // 4
+    keep = np.zeros((nin, 6), bool)
     for rg in range(6):
-        keep[rng.choice(N_A // 4, 42, replace=False), rg] = True
+        keep[rng.choice(nin, GRUB_EVEN_BLOCKS[na], replace=False), rg] = True
     return keep
 
 
-def _grua_skew(rng, gate, q):
+def _grua_skew(rng, gate, q, na=N_A):
     """GRU_A blocks kept above one block-energy threshold per gate (Sparsify, training_tf2/lpcnet.py:96-116) of weights with
     strong and weak neuron groups and inputs, so the list lengths are skewed; then the list shapes the kernels' walkers can get
     wrong are forced on fixed row groups (the same groups in every gate):
-      0, 6, 7   empty          1, 2, 3   one, two and three blocks (partial quads)
-      4         8 blocks all of one (pos/4)&3 class (put_quads must repeat a class)
-      5, 8..15  include the last column block, pos = NA-4"""
-    nin, nout = N_A // 4, N_A // 8
+      0, 6, 7   empty (at 128 units, where each compute warp owns one neuron group, three warps walk no GRU_A quad at all)
+      1, 2, 3   one, two and three blocks (partial quads)
+      4         8 blocks all of one (pos/4)&3 class (put_quads must repeat a class): column blocks 4*(2..9)+c, at 128 units
+                (32 column blocks, 8 per class) 4*(0..7)+c
+      5, 8..15  include the last column block, pos = na-4"""
+    nin, nout = na // 4, na // 8
     e = (q.reshape(nin, 4, nout, 8).astype(np.float64) ** 2).sum(axis=(1, 3))
     e *= np.exp(rng.normal(0.0, 1.2, size=(1, nout))) * np.exp(rng.normal(0.0, 0.6, size=(nin, 1)))
     keep = e > np.quantile(e, 1.0 - (0.075, 0.075, 0.25)[gate])
@@ -476,7 +483,7 @@ def _grua_skew(rng, gate, q):
         keep[:, rg] = False
         keep[rng.choice(nin, n, replace=False), rg] = True
     keep[:, 4] = False
-    keep[4 * np.arange(2, 10) + (gate + 1) % 4, 4] = True
+    keep[4 * (np.arange(8) + (0 if na == 128 else 2)) + (gate + 1) % 4, 4] = True
     keep[nin - 1, 5] = True
     keep[nin - 1, 8:16] = True
     return keep
@@ -516,8 +523,9 @@ FAST_CVT_LIMIT = 4194304.0 * 0.99      # model.cu: conversion-free rounding whil
 
 
 STRESS_SEED = 2100
-# Stress models (all GRU_A 384, the default header: the compiled reference builds A and B load them at run time).  name ->
-# make_model() hooks; "cvt" sets the loader's accumulator bound (cvt_bound) to that value by raising a few biases.
+# Stress models, made at each GRU_A size of STRESS_NA (the default header and those of the na256 / na128 variants: the compiled
+# reference builds A and B of that header load them at run time).  name -> make_model() hooks; "cvt" sets the loader's
+# accumulator bound (cvt_bound) to that value by raising a few biases.
 STRESS = {
     "grub_split": dict(grub_keep=_grub_split),
     "grub_even":  dict(grub_keep=_grub_even),
@@ -529,37 +537,70 @@ STRESS = {
 }
 
 
-def make_stress_model(name):
-    """(arrays_common, arrays_int8, arrays_float) of STRESS[name]; each model has its own seed."""
-    kw = dict(STRESS[name])
+STRESS_NA = (384, 256, 128)     # every STRESS model exists at each GRU_A size the kernels are built for
+
+
+def _grua_full(rng, gate, q, na=N_A):
+    """A uniform random GRU_A mask of density 0.485: at 256 units the int8 image then leaves room for only 32 of the 64 dual_fc
+    rows (the loader gives up the others by itself), while the accumulator bound stays far inside the conversion-free rounding's."""
+    return rng.random((na // 4, na // 8)) < 0.485
+
+
+# Stress models made at one size only: name -> (na, make_model() hooks).  At 384 units `skew` already fills the image.
+STRESS_AT = {
+    "full": (256, dict(grua_keep=_grua_full)),
+}
+
+
+def stress_names(na=N_A):
+    """The stress models that exist with `na` GRU_A units."""
+    return list(STRESS) + [n for n, (w, _) in STRESS_AT.items() if w == na]
+
+
+def make_stress_model(name, na=N_A):
+    """(arrays_common, arrays_int8, arrays_float) of STRESS[name] (or STRESS_AT[name]) with `na` GRU_A units; each model has its
+    own seed (the same at every size)."""
+    names = list(STRESS) + list(STRESS_AT)
+    if name in STRESS_AT:
+        assert na == STRESS_AT[name][0], (name, na)
+    kw = dict(STRESS[name] if name in STRESS else STRESS_AT[name][1])
     target = kw.pop("cvt", None)
-    common, only8, onlyf = make_model(STRESS_SEED + list(STRESS).index(name), **kw)
+    for hook in ("grub_keep", "grua_keep"):
+        if hook in kw:
+            kw[hook] = functools.partial(kw[hook], na=na)
+    common, only8, onlyf = make_model(STRESS_SEED + names.index(name), na=na, **kw)
     if target is not None:
         # the recurrent bias of the candidate gate of neuron group 0 (alternating signs, bias and su-bias alike) becomes the
         # largest one, so that cvt_bound() == target: these neurons' accumulators are the largest the bound allows
         arrs = {n: a for n, _, a in common + only8}
-        rows = 2 * N_A + np.arange(8)
+        rows = 2 * na + np.arange(8)
         sub, bias = arrs["sparse_gru_a_subias"], arrs["sparse_gru_a_bias"]
         sub[1, rows] = bias[1, rows] = 0.0
         rest = np.abs(sub[1]).max()
-        b = np.float32(rest + (target - cvt_bound(arrs)) / (1.01 * 128.0 * 127.0))
+        b = np.float32(rest + (target - cvt_bound(arrs, na)) / (1.01 * 128.0 * 127.0))
         assert b > rest
         sub[1, rows] = bias[1, rows] = b * np.where(np.arange(8) % 2, -1.0, 1.0).astype(np.float32)
     return common, only8, onlyf
 
 
-def stress_arrays(name, kind="int8"):
-    common, only8, onlyf = make_stress_model(name)
+def stress_arrays(name, kind="int8", na=N_A):
+    common, only8, onlyf = make_stress_model(name, na)
     return {n: a for n, _, a in common + (only8 if kind == "int8" else onlyf)}
 
 
+def stress_blob_name(name, kind, na=N_A):
+    """File name of a stress blob: stress_<name>_<kind>.bin at 384 units, stress_<name>_na<na>_<kind>.bin otherwise."""
+    return "stress_%s_%s.bin" % (name if na == N_A else "%s_na%d" % (name, na), kind)
+
+
 def generate_stress(out):
-    """Writes stress_<name>_{int8,float}.bin for every STRESS model into `out`."""
+    """Writes the int8 and float blobs of every STRESS model at every size of STRESS_NA into `out`."""
     os.makedirs(out, exist_ok=True)
-    for name in STRESS:
-        common, only8, onlyf = make_stress_model(name)
-        write_blob(os.path.join(out, "stress_%s_int8.bin" % name), common + only8)
-        write_blob(os.path.join(out, "stress_%s_float.bin" % name), common + onlyf)
+    for na in STRESS_NA:
+        for name in stress_names(na):
+            common, only8, onlyf = make_stress_model(name, na)
+            write_blob(os.path.join(out, stress_blob_name(name, "int8", na)), common + only8)
+            write_blob(os.path.join(out, stress_blob_name(name, "float", na)), common + onlyf)
     return out
 
 

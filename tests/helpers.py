@@ -40,10 +40,11 @@ STRESS_DIR = GEN + "_stress"
 
 
 @functools.lru_cache(None)
-def stress_blob(name, kind="int8"):
-    """Blob of one of gen_model.STRESS (kind int8 | float), generated into oracle/_gen_stress on first use."""
+def stress_blob(name, kind="int8", na=384):
+    """Blob of one of gen_model.STRESS (kind int8 | float) with `na` GRU_A units (gen_model.STRESS_NA), generated into
+    oracle/_gen_stress on first use."""
     import gen_model
-    path = os.path.join(STRESS_DIR, "stress_%s_%s.bin" % (name, kind))
+    path = os.path.join(STRESS_DIR, gen_model.stress_blob_name(name, kind, na))
     if not os.path.exists(path):
         gen_model.generate_stress(STRESS_DIR)
     return open(path, "rb").read()

@@ -37,10 +37,18 @@ def test_variant_matches_reference_golden(eng, tag, kind, build):
     assert _first_diff(got, gold) is None, "first mismatch (stream, sample) = %s" % (_first_diff(got, gold),)
 
 
+# streams per CTA of each case, pinned: on its own a batch this small is spread over the SMs one stream per CTA
+VARIANT_SPC = {("int8", 70): "32", ("float", 37): "32"}
+
+
 @pytest.mark.parametrize("tag", TAGS)
 @pytest.mark.parametrize("kind,n", [("int8", 70), ("int8", 9), ("float", 37), ("float", 3)])
-def test_variant_batches_match_oracle(eng, tag, kind, n):
-    """two-half and half-A-only schedules of the int8 kernel, lane==stream and neuron-per-lane float kernels, ragged CTAs"""
+def test_variant_batches_match_oracle(eng, monkeypatch, tag, kind, n):
+    """int8: 70 streams at 32 per CTA (two halves; CTAs of 32, 32 and 6) and 9 on the automatic schedule (one half, one live
+    slot per CTA); float: 37 streams at 32 per CTA (the lane==stream kernel, a ragged CTA of 5) and 3 on the automatic schedule
+    (the neuron-per-lane kernel)"""
+    if (kind, n) in VARIANT_SPC:
+        monkeypatch.setenv("LPCNET_B200_STREAMS_PER_CTA", VARIANT_SPC[(kind, n)])
     T = 9
     f = make_feature_batch(range(400, 400 + n), T)
     b = eng.Batch(n, H.blob(kind, tag), config=H.model_config(tag))
