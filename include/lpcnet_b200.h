@@ -276,9 +276,9 @@ LPCNET_EXPORT int lpcnet_b200_debug_image(const unsigned char *blob, int len, un
 /* Same for the second image of float models (the neuron-per-lane kernel used for small batches); layout[17]. */
 LPCNET_EXPORT int lpcnet_b200_debug_image_n(const unsigned char *blob, int len, unsigned char *out, size_t cap,
                                             uint32_t *layout);
-/* Test hook: evaluate the engine's two implementations of the reference's _mm256_rcp_ps emulation (memory table /
- * table-free arithmetic) on n host floats. */
-LPCNET_EXPORT int lpcnet_b200_debug_rcp(LPCNetB200Batch *b, const float *x, float *out_table, float *out_arith, int n);
+/* Test hook: evaluate the engine's emulation of the reference's _mm256_rcp_ps (the per-sample kernels' table) on n host
+ * floats. */
+LPCNET_EXPORT int lpcnet_b200_debug_rcp(LPCNetB200Batch *b, const float *x, float *out, int n);
 /* Test hook: the conditioning network's full-range _mm256_rcp_ps emulation (zeros, denormals, infinities, NaN, |x| >= 2^126)
  * and its tanh8_approx with the reference's NaN order on n host floats. */
 LPCNET_EXPORT int lpcnet_b200_debug_tanh_x86(LPCNetB200Batch *b, const float *x, float *out_rcp, float *out_tanh, int n);

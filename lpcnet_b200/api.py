@@ -67,7 +67,7 @@ def lib():
     L.lpcnet_b200_batch_is_float.argtypes = [c_p]
     L.lpcnet_b200_batch_get_state.argtypes = [c_p, ctypes.c_int, c_p, c_p, c_p, c_p, c_p]
     L.lpcnet_b200_debug_frame_network.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
-    L.lpcnet_b200_debug_rcp.argtypes = [c_p, c_p, c_p, c_p, ctypes.c_int]
+    L.lpcnet_b200_debug_rcp.argtypes = [c_p, c_p, c_p, ctypes.c_int]
     L.lpcnet_b200_debug_tanh_x86.argtypes = [c_p, c_p, c_p, c_p, ctypes.c_int]
     L.lpcnet_b200_set_default_model.argtypes = [ctypes.c_char_p, ctypes.c_int, ctypes.c_float]
     L.lpcnet_b200_set_default_codebooks.argtypes = [c_p, ctypes.c_size_t]
@@ -532,12 +532,12 @@ class Batch:
         return ga, gb, lpc
 
     def debug_rcp(self, x):
-        """(table result, table-free result) of the engine's _mm256_rcp_ps emulation for an array of floats."""
+        """The engine's _mm256_rcp_ps emulation (the per-sample kernels' table) for an array of floats."""
         x = np.ascontiguousarray(x, dtype=np.float32)
-        a = np.zeros_like(x); b = np.zeros_like(x)
-        if self._L.lpcnet_b200_debug_rcp(self._h, x.ctypes.data, a.ctypes.data, b.ctypes.data, int(x.size)) != 0:
+        a = np.zeros_like(x)
+        if self._L.lpcnet_b200_debug_rcp(self._h, x.ctypes.data, a.ctypes.data, int(x.size)) != 0:
             raise LPCNetB200Error(_err())
-        return a, b
+        return a
 
     def debug_tanh_x86(self, x):
         """(rcp, tanh) of the conditioning network's full-range activation for an array of floats."""

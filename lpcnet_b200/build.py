@@ -55,7 +55,8 @@ def needs_build():
 
 
 def build_variant(name, defines):
-    """Tuning aid: build lpcnet_b200/variants/lib_<name>.so with extra -D flags (e.g. LPCNET_NWC=12)."""
+    """Instrumented build: lpcnet_b200/variants/lib_<name>.so with extra -D flags, LPCNET_TRACE (clock64 timeline of CTA 0,
+    tools/trace_run.py) or LPCNET_ARRIVE_ALL (every lane arrives on the mbarriers, for a race checker)."""
     vdir = os.path.join(HERE, "variants")
     log = []
     os.makedirs(vdir, exist_ok=True)

@@ -1078,26 +1078,23 @@ int lpcnet_b200_debug_image(const unsigned char *blob, int len, unsigned char *o
     return r;
 }
 
-// Test hook: the two device implementations of the reference's _mm256_rcp_ps (table in memory / table-free arithmetic)
-// on n host floats.
-__global__ void debug_rcp_kernel(const float *x, float *out_table, float *out_arith, int n, const uint16_t *tab16)
+// Test hook: the device implementation of the reference's _mm256_rcp_ps (the table in memory) on n host floats.
+__global__ void debug_rcp_kernel(const float *x, float *out, int n, const uint16_t *tab16)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    out_table[i] = rcp_emul(x[i], tab16);
-    out_arith[i] = rcp_emul(x[i], RcpArith());
+    out[i] = rcp_emul(x[i], tab16);
 }
-int lpcnet_b200_debug_rcp(LPCNetB200Batch *b, const float *x, float *out_table, float *out_arith, int n)
+int lpcnet_b200_debug_rcp(LPCNetB200Batch *b, const float *x, float *out, int n)
 {
     if (!b || n <= 0) { set_error("debug_rcp: bad arguments"); return -1; }
     CK(cudaSetDevice(b->device));
     float *d = nullptr;
-    CK(cudaMalloc(&d, (size_t)3 * n * sizeof(float)));
+    CK(cudaMalloc(&d, (size_t)2 * n * sizeof(float)));
     CK(cudaMemcpy(d, x, (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
-    debug_rcp_kernel<<<(n + 255) / 256, 256, 0, b->stream>>>(d, d + n, d + 2 * n, n, b->model.rcp16);
+    debug_rcp_kernel<<<(n + 255) / 256, 256, 0, b->stream>>>(d, d + n, n, b->model.rcp16);
     CK(cudaStreamSynchronize(b->stream));
-    CK(cudaMemcpy(out_table, d + n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(out_arith, d + 2 * n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(out, d + n, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
     cudaFree(d);
     return 0;
 }

@@ -37,27 +37,6 @@ __device__ __forceinline__ float rcp_emul(float x, RcpShared tab)
     return __uint_as_float(t - (u & 0x7F800000u));
 }
 
-// The same function WITHOUT a table (no shared-memory traffic: the look-up above costs ~3.4 bank-conflicted wavefronts
-// per warp, the binding unit of the per-sample kernel).  The table has the closed form T[k] = rint(2^25/d) * 2^-13 with
-// d = 2k + 4097 (tests/test_oracle.py): d is formed exactly as a float from the top 11 mantissa bits, MUFU.RCP gives
-// 2^25/d to within +-1 after rounding, and the EXACT residual q*d - 2^25 (an integer below 2^24, so one FMA computes
-// it without error) decides the +-1 correction; d is odd, so there are no ties.  Checked against the table for every
-// k, exponent and sign of the low bits by tests/test_gpu_parity.py::test_arithmetic_rcpps_matches_table.
-struct RcpArith {};
-__device__ __forceinline__ float rcp_emul(float x, RcpArith)
-{
-    const uint32_t u = __float_as_uint(x);
-    const float d = __uint_as_float((u & 0x007FF000u) | 0x45800800u);        // 4097 + 2k, exact
-    float y;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(d));
-    float q = __fsub_rn(__fmaf_rn(y, 33554432.f, 12582912.f), 12582912.f);   // rint(y * 2^25)
-    const float e = __fmaf_rn(q, d, -33554432.f);                           // q*d - 2^25, exact
-    const float dh = __fmul_rn(d, 0.5f);
-    q = __fadd_rn(__fsub_rn(q, e > dh ? 1.f : 0.f), e < -dh ? 1.f : 0.f);
-    // T[k] + 0x3f800000 - exponent(x):  q in [4097, 8191] is 0x45800000 + ((q - 4096) << 11) as a float pattern
-    return __uint_as_float(__float_as_uint(q) + 0x39000000u - (u & 0x7F800000u));
-}
-
 // tanh8_approx (vec_avx.h:393-411)
 template <typename TAB>
 __device__ __forceinline__ float tanh_approx(float x, TAB tab16)
@@ -116,36 +95,6 @@ __device__ __forceinline__ float sigmoid_approx(float x, TAB tab16)
     den = rcp_emul(den, tab16);
     num = __fmaf_rn(num, den, 0.5f);
     return fmaxf(0.f, fminf(1.f, num));
-}
-
-// ---- pairs of fp32 values (the two neurons of a lane) ----
-// Used for the pieces of the activations where both neurons of a lane run the same op.  sm_90 has no packed fp32
-// instructions: a pair is two registers and every pair op is two round-to-nearest intrinsics, which the compiler
-// never contracts (so a mul followed by an add keeps both roundings, as in the reference).
-struct f32x2 { float lo, hi; };
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return {lo, hi}; }
-__device__ __forceinline__ void upk2(f32x2 v, float &lo, float &hi) { lo = v.lo; hi = v.hi; }
-__device__ __forceinline__ f32x2 k2(float c) { return pk2(c, c); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return {__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return {__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return {__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
-// 1 - z for two values: fma(z, -1, 1) = rn(1 - z)
-__device__ __forceinline__ f32x2 one_minus2(f32x2 z) { return fma2(z, k2(-1.f), k2(1.f)); }
-// numerator * x and denominator of the rational approximations (before the reciprocal), two values at a time:
-// X2 = x*x; num = fma(fma(N2,X2,N1),X2,N0) * x; den = fma(fma(D2,X2,D1),X2,D0)          (vec_avx.h:393-440)
-__device__ __forceinline__ void rational2(f32x2 x, float N0, float N1, float N2, float D0, float D1, float D2, f32x2 &num, f32x2 &den)
-{
-    const f32x2 X2 = mul2(x, x);
-    num = fma2(fma2(k2(N2), X2, k2(N1)), X2, k2(N0));
-    den = fma2(fma2(k2(D2), X2, k2(D1)), X2, k2(D0));
-    num = mul2(num, x);
-}
-#define LPCNET_SIGMOID_COEF 238.13200378f, 6.02452230f, 0.00950985f, 952.72399902f, 103.34200287f, 0.74287558f
-#define LPCNET_TANH_COEF 952.52801514f, 96.39235687f, 0.60863042f, 952.72399902f, 413.36801147f, 11.88600922f
-// (float)acc * SCALE_1 for two biased accumulators (see acc_init_t below): add -> mul, safe to pack
-__device__ __forceinline__ f32x2 acc_finish2(int a0, int a1)
-{
-    return mul2(add2(pk2(__int_as_float(a0), __int_as_float(a1)), k2(-12582912.f)), k2(LPCNET_SCALE_1));
 }
 
 // vector_ps_to_epi8 (vec_avx.h:321-336): u8 = sat(rne(fma(x,127,127)))
@@ -231,13 +180,5 @@ __device__ __forceinline__ uint32_t kiss99_rand(Kiss99 &t)
 }
 
 __device__ __forceinline__ float4 ldg4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
-// read-only 16-byte load that does not allocate in L1 (the gathered embedding rows have no reuse there; the small L1 left
-// beside 227 KB of shared memory is kept for the sampler's dual_fc rows)
-__device__ __forceinline__ float4 ldg4_stream(const float *p)
-{
-    float4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
 
 }  // namespace lpcnet_b200

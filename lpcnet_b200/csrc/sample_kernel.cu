@@ -12,9 +12,9 @@
 // One CTA = 32 independent streams on one SM, stepped as two HALVES of 16 streams that run half a sample apart:
 // a GRU step cannot start before the previous sample of the same stream has been drawn and its embedding rows gathered,
 // so while that serial tail (sampler -> indices -> gather) runs for one half, the compute warps work on the other half.
-// NWC + NWP + 1 warps:
+// NWC + NWP + 2 = 16 + 6 + 2 warps (engine.h):
 //
-//   NWC compute warps own 48/NWC neuron groups (8 neurons x {z,r,h}) of GRU_A each.  The integer GEMVs S = W.q(h) of a
+//   NWC compute warps own NGRP/NWC neuron groups (8 neurons x {z,r,h}) of GRU_A each.  The integer GEMVs S = W.q(h) of a
 //                     half are small GEMMs and run on the tensor cores: mma.sync m16n8k16 (u8 x s8 -> s32, exact, so the
 //                     summation order is free): M = the 16 streams of the half, N = the 8 neurons of a row group, K = four
 //                     8x4 weight blocks ("quad") whose column blocks may be anywhere (block-sparse): the A fragment of lane
@@ -43,50 +43,7 @@
 #ifndef LPCNET_NA
 #define LPCNET_NA 384          // GRU_A units this translation unit is compiled for (lpcnet_b200/build.py compiles one per supported size)
 #endif
-#include "engine.h"
-#include "devmath.cuh"
-
-#ifndef LPCNET_RCP_ARITH
-#define LPCNET_RCP_ARITH 0     // bit mask of the GRU_A gates (1: r, 2: z, 4: candidate) whose activations use the table-free RCPPS of devmath.cuh
-                               // instead of the shared-memory table (exact either way).  The table costs ~3.4 bank-conflicted wavefronts per
-                               // look-up on the LSU pipe, the arithmetic form 8 more issue slots
-#endif
-#ifndef LPCNET_PACK_ACT
-#define LPCNET_PACK_ACT 1      // GRU_A activations: also the mul -> add pieces are written as pair ops (devmath.cuh)
-#endif
-#ifndef LPCNET_COND_TMA
-#define LPCNET_COND_TMA 0      // 1: the conditioning rows of a gather tile come by TMA ahead of the sampled indices (gather_half_tma below): the tile
-                               // fill drops from 3.7 k to 2.7 k cycles, but the same bytes then cross the shared-memory port twice (TMA write + LDS) and
-                               // the step did not get shorter; kept as a build option (bit-exact in the
-                               // golden / oracle / grid-shape tests of the 384-unit model; the 128- and 256-unit builds of it have not been run)
-#endif
-#ifndef LPCNET_FCW_PREFETCH
-#define LPCNET_FCW_PREFETCH 0  // 1: the sampler prefetches the dual_fc rows of the tree levels that are read from global memory into L1 two levels
-                               // ahead (CCTL.PF1); off
-#endif
-#ifndef LPCNET_EXPERIMENT
-#define LPCNET_EXPERIMENT 0    // timing experiments only (wrong output): 1 = sampler delayed by 1000 cycles, 2 = sampler skips the two lowest tree levels
-#endif
-#ifndef LPCNET_GRUB_FIRST
-#define LPCNET_GRUB_FIRST 3    // bit 0 / bit 1: GRU_B of half A / half B runs right after the half's activations, before the other half's first GEMVs
-                               // (the GRU_B state is what the half's sampler waits for)
-#endif
-#ifndef LPCNET_FIN_FIRST_WARP
-#define LPCNET_FIN_FIRST_WARP (NWC - NFIN)   // the NFIN compute warps that finish GRU_B: the LAST ones, which carry no (or the least) GRU_B GEMV work
-#endif
-#ifndef LPCNET_TREE_PAR
-#define LPCNET_TREE_PAR 0      // 1: sampler evaluates the seven nodes of the first three tree levels side by side (see the sampler loop); bit-exact but
-                               // slower: four more dot products per sample and more spilled state in the
-                               // sampler cost more than the two serial rounds they save
-#endif
-#ifndef LPCNET_GATHER_NOALLOC
-#define LPCNET_GATHER_NOALLOC 0
-#endif
-#if LPCNET_GATHER_NOALLOC
-#define GLD ldg4_stream
-#else
-#define GLD ldg4
-#endif
+#include "sample_common.cuh"
 
 // tuning builds (-DLPCNET_TRACE): clock64 stamps of CTA 0 for samples 200..207 of a launch
 #ifdef LPCNET_TRACE
@@ -115,26 +72,8 @@ enum {
     BAR_HB = 3       // (+ half) finishing warps arrive, sampler waits: GRU_B state of the half's sample is in hBs
 };
 constexpr int CNT_C = NWC * 32, CNT_HB = NFIN * 32 + 32;
-constexpr int FIN0 = LPCNET_FIN_FIRST_WARP;
-__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+constexpr int FIN0 = NWC - NFIN;     // the NFIN compute warps that finish GRU_B: the LAST ones, which carry no (or the least) GRU_B GEMV work
 
-__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// ---- TMA bulk copy global -> shared, completion on an mbarrier ----
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -154,18 +93,6 @@ __device__ __forceinline__ void warp_arrive(uint32_t bar, int lane)
     if (lane == 0) mbar_arrive(bar);
 }
 #endif
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
 
 __device__ __forceinline__ uint32_t lds32(uint32_t addr)
 {
@@ -277,7 +204,7 @@ __device__ __forceinline__ void gather_half(float *__restrict__ G, const float *
         constexpr int NCH = NA / 128;
         float4 a[NCH], b[NCH], d[NCH], e[NCH];
 #pragma unroll
-        for (int j = 0; j < NCH; j++) { a[j] = GLD(c + 128 * j); b[j] = GLD(e0 + 128 * j); d[j] = GLD(e1 + 128 * j); e[j] = GLD(e2 + 128 * j); }
+        for (int j = 0; j < NCH; j++) { a[j] = ldg4(c + 128 * j); b[j] = ldg4(e0 + 128 * j); d[j] = ldg4(e1 + 128 * j); e[j] = ldg4(e2 + 128 * j); }
         float *g = G + si * GIN_ROW + lane * 4;
 #pragma unroll
         for (int j = 0; j < NCH; j++) {
@@ -287,76 +214,6 @@ __device__ __forceinline__ void gather_half(float *__restrict__ G, const float *
             r.z = __fadd_rn(__fadd_rn(__fadd_rn(a[j].z, b[j].z), d[j].z), e[j].z);
             r.w = __fadd_rn(__fadd_rn(__fadd_rn(a[j].w, b[j].w), d[j].w), e[j].w);
             *reinterpret_cast<float4 *>(g + 128 * j) = r;
-        }
-    }
-}
-
-// The same tile with the conditioning row prefetched.  Of the four rows that make a tile row only three depend on the indices the
-// sampler has just produced; the conditioning row is known a whole frame ahead.  Producer 0 therefore starts one TMA bulk copy per
-// live tile row (NA*4 bytes, straight into the row's place in the tile) for all three tiles of a half-step BEFORE it waits for the
-// indices (kernel body), and the gather proper adds the three embedding rows in place:
-//   G[si][k] = ((G[si][k] + E_sig[a][k]) + E_pred[b][k]) + E_exc[c][k]
-// Three dependent loads per element instead of four: the 12 LDG.128 a lane keeps in flight cover FOUR 128-column row pieces instead of
-// three, and a tile is two latency-bound load batches per producer instead of three (the tile fill is on the serial chain of a
-// sample: indices -> tiles -> activations -> GRU_B -> sampler -> indices).  Work split: rows 0..FULL_ROWS-1 are dealt whole, row
-// p + NWP*b to producer p in batch b; the pieces of the remaining rows go round the producers, one per batch.
-// Rows >= late0 (only for the r tile, which takes the slot the half's GRU_B state scratch lives in: engine.h, Geom::late_row0) could
-// not be prefetched (the sampler may still be reading the scratch): their conditioning piece is loaded here like the others.
-constexpr int FULL_ROWS = (HALF / NWP) * NWP, GATHER_BATCHES = HALF / NWP;
-static_assert((HALF - FULL_ROWS) * (NA / 128) <= GATHER_BATCHES * NWP, "one piece of the shared rows per producer and batch");
-template <bool ONE>
-__device__ __forceinline__ void gather_half_tma(float *__restrict__ G, const float *__restrict__ cond_f, int n, int cta_s0, int hh, int spc, int nl, int late0,
-                                                const float *__restrict__ emb_sig, const float *__restrict__ emb_pred,
-                                                const float *__restrict__ emb_exc, const int *__restrict__ idx_h,
-                                                int gate, int p, int lane)
-{
-    constexpr int NCH = NA / 128;
-    const int col = gate * NA + lane * 4;
-#pragma unroll 1
-    for (int b = 0; b < GATHER_BATCHES; b++) {
-        const int r = p + NWP * b;                               // whole row
-        const int c = p + NWP * b, rs = FULL_ROWS + c / NCH, cj = c % NCH;   // piece cj of shared row rs
-        const bool hasr = r < nl, hass = c < (HALF - FULL_ROWS) * NCH && rs < nl, lates = hass && rs >= late0;
-        float4 B[NCH], D[NCH], E[NCH], sb, sd, se, sc;
-        if (hasr) {
-            const float *e0 = emb_sig + idx_h[r] * (3 * NA) + col;
-            const float *e1 = emb_pred + idx_h[HALF + r] * (3 * NA) + col;
-            const float *e2 = emb_exc + idx_h[2 * HALF + r] * (3 * NA) + col;
-#pragma unroll
-            for (int j = 0; j < NCH; j++) { B[j] = GLD(e0 + 128 * j); D[j] = GLD(e1 + 128 * j); E[j] = GLD(e2 + 128 * j); }
-        }
-        if (hass) {
-            sb = GLD(emb_sig + idx_h[rs] * (3 * NA) + col + 128 * cj);
-            sd = GLD(emb_pred + idx_h[HALF + rs] * (3 * NA) + col + 128 * cj);
-            se = GLD(emb_exc + idx_h[2 * HALF + rs] * (3 * NA) + col + 128 * cj);
-            if (lates) {
-                bool live;
-                const int sg = slot_stream<ONE>(cta_s0, hh, rs, spc, n, live);
-                sc = GLD(cond_row(cond_f, n, gate, sg) + lane * 4 + 128 * cj);
-            }
-        }
-        if (hasr) {
-            float *g = G + r * GIN_ROW + lane * 4;
-#pragma unroll
-            for (int j = 0; j < NCH; j++) {
-                const float4 a = *reinterpret_cast<const float4 *>(g + 128 * j);
-                float4 o;
-                o.x = __fadd_rn(__fadd_rn(__fadd_rn(a.x, B[j].x), D[j].x), E[j].x);
-                o.y = __fadd_rn(__fadd_rn(__fadd_rn(a.y, B[j].y), D[j].y), E[j].y);
-                o.z = __fadd_rn(__fadd_rn(__fadd_rn(a.z, B[j].z), D[j].z), E[j].z);
-                o.w = __fadd_rn(__fadd_rn(__fadd_rn(a.w, B[j].w), D[j].w), E[j].w);
-                *reinterpret_cast<float4 *>(g + 128 * j) = o;
-            }
-        }
-        if (hass) {
-            float *g = G + rs * GIN_ROW + lane * 4 + 128 * cj;
-            if (!lates) sc = *reinterpret_cast<const float4 *>(g);
-            float4 o;
-            o.x = __fadd_rn(__fadd_rn(__fadd_rn(sc.x, sb.x), sd.x), se.x);
-            o.y = __fadd_rn(__fadd_rn(__fadd_rn(sc.y, sb.y), sd.y), se.y);
-            o.z = __fadd_rn(__fadd_rn(__fadd_rn(sc.z, sb.z), sd.z), se.z);
-            o.w = __fadd_rn(__fadd_rn(__fadd_rn(sc.w, sb.w), sd.w), se.w);
-            *reinterpret_cast<float4 *>(g) = o;
         }
     }
 }
@@ -380,9 +237,8 @@ struct ComputeCtx {
 
 // One GRU_A + GRU_B step of half H (16 streams).  k0 = index of the half-step's first tile fill (gate r; z and h follow).
 // A half-step of the compute warps is three pieces:  gemv_rh<H>  |  activations<H> (ends by ARRIVING on MB_X[H])  |  grub<H> (WAITS on MB_X[H]).
-// grub<H> used to run only after the other half's gemv_rh, so that no CTA-wide barrier was waited for right after it was armed; but the
-// GRU_B state is what the half's sampler waits for, i.e. it is on the serial chain of a sample, while a warp that waits at the barrier only
-// gives its issue slots to the others: LPCNET_GRUB_FIRST (default) runs it right behind the activations.
+// grub<H> runs right behind the half's activations, before the other half's gemv_rh: the GRU_B state is what the half's sampler waits for,
+// i.e. it is on the serial chain of a sample, while a warp that waits at the barrier only gives its issue slots to the others.
 
 // GEMVs of the candidate and reset gates of half H (need only the previous state)
 template <int H>
@@ -405,33 +261,15 @@ template <int H, bool FAST>
 __device__ __forceinline__ void activations(const ComputeCtx &C, float (&h)[GPW][4], int (&Sh)[GPW][4], int (&Sg)[GPW][4], uint32_t k0, int cur)
 {
     uint8_t *smem = C.smem;
-    const int gid = C.gid, t = C.t, lane = C.lane, warp = C.warp;
-    // per-gate choice of the RCPPS implementation (LPCNET_RCP_ARITH mask)
-#if LPCNET_RCP_ARITH & 1
-    const RcpArith rcp_r = RcpArith();
-#else
-    const RcpShared rcp_r = C.rcp;
-#endif
-#if LPCNET_RCP_ARITH & 2
-    const RcpArith rcp_z = RcpArith();
-#else
-    const RcpShared rcp_z = C.rcp;
-#endif
-#if LPCNET_RCP_ARITH & 4
-    const RcpArith rcp_h = RcpArith();
-#else
-    const RcpShared rcp_h = C.rcp;
-#endif
-    const int nxt = cur ^ 1;
+    const int gid = C.gid, lane = C.lane;
+    const RcpShared rcp = C.rcp;
     const uint32_t xs_cur = C.xs0 + cur * XS_BYTES, lc = C.gid8 | (H << 6);
-    uint8_t *xs_nxt = smem + SM_XS + nxt * XS_BYTES;
+    uint8_t *xs_nxt = smem + SM_XS + (cur ^ 1) * XS_BYTES;
     const uint32_t kr = k0, kz = k0 + 1, kh = k0 + 2;
     const float *tile_r = reinterpret_cast<const float *>(smem + SM_TILES + (kr & 3) * TILE_BYTES) + gid * GIN_ROW;
     const float *tile_z = reinterpret_cast<const float *>(smem + SM_TILES + (kz & 3) * TILE_BYTES) + gid * GIN_ROW;
-    uint8_t *tile_hb = smem + SM_TILES + (kh & 3) * TILE_BYTES;
-    const float *tile_h = reinterpret_cast<const float *>(tile_hb) + gid * GIN_ROW;
+    const float *tile_h = reinterpret_cast<const float *>(smem + SM_TILES + (kh & 3) * TILE_BYTES) + gid * GIN_ROW;
     const uint32_t mb_full = smem_u32(smem + MB_FULL), mb_empty = smem_u32(smem + MB_EMPTY);
-    (void)t; (void)warp; (void)rcp_r; (void)rcp_z; (void)rcp_h; (void)nxt; (void)xs_cur; (void)lc; (void)xs_nxt; (void)tile_r; (void)tile_z; (void)tile_h; (void)mb_full; (void)mb_empty; (void)lane;
     // ---- reset gate r (nnet.c:431-435) with the gathered input term; keep rec_h * r (nnet.c:436-440) ----
     mbar_wait(mb_full + 8 * (kr & 3), (kr >> 2) & 1);
 #pragma unroll
@@ -444,50 +282,13 @@ __device__ __forceinline__ void activations(const ComputeCtx &C, float (&h)[GPW]
         for (int jj = 0; jj < 2; jj++) {
             const float2 gv = *reinterpret_cast<const float2 *>(tile_r + 8 * jj * GIN_ROW + C.gcol[sl]);
             const float gin[2] = {gv.x, gv.y};
-            if constexpr (FAST) {
-                int a[2], ah[2];
-#if LPCNET_PACK_ACT
-                {   // both neurons of the lane at a time
-                    const f32x2 hv2 = pk2(h[sl][2 * jj], h[sl][2 * jj + 1]);
-                    float a0, a1, b0, b1;
-                    upk2(add2(mul2(add2(add2(mul2(pk2(dr.x, dr.y), hv2), pk2(br.x, br.y)), pk2(gv.x, gv.y)), k2(LPCNET_SCALE)), k2(LPCNET_CVT_MAGIC)), a0, a1);
-                    upk2(add2(mul2(add2(mul2(pk2(dh.x, dh.y), hv2), pk2(bh.x, bh.y)), k2(LPCNET_SCALE)), k2(LPCNET_CVT_MAGIC)), b0, b1);
-                    a[0] = __float_as_int(a0) + Sg[sl][2 * jj]; a[1] = __float_as_int(a1) + Sg[sl][2 * jj + 1];
-                    ah[0] = __float_as_int(b0) + Sh[sl][2 * jj]; ah[1] = __float_as_int(b1) + Sh[sl][2 * jj + 1];
-                }
-#else
-                // mul -> add pieces scalar, the rest two neurons at a time (devmath.cuh)
 #pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const float hv = h[sl][2 * jj + i];
-                    a[i] = acc_init_t<true>(__fadd_rn(__fadd_rn(bri[i], __fmul_rn(dri[i], hv)), gin[i])) + Sg[sl][2 * jj + i];
-                    ah[i] = acc_init_t<true>(__fadd_rn(bhi[i], __fmul_rn(dhi[i], hv))) + Sh[sl][2 * jj + i];
-                }
-#endif
-                f32x2 num, den;
-                rational2(acc_finish2(a[0], a[1]), LPCNET_SIGMOID_COEF, num, den);
-                float n0, n1, d0, d1, rh0, rh1;
-                upk2(num, n0, n1); upk2(den, d0, d1);
-                const float r0 = fmaxf(0.f, fminf(1.f, __fmaf_rn(n0, rcp_emul(d0, rcp_r), 0.5f)));
-                const float r1 = fmaxf(0.f, fminf(1.f, __fmaf_rn(n1, rcp_emul(d1, rcp_r), 0.5f)));
-#if LPCNET_PACK_ACT
-                upk2(mul2(acc_finish2(ah[0], ah[1]), pk2(r0, r1)), rh0, rh1);
-                Sh[sl][2 * jj] = __float_as_int(rh0);
-                Sh[sl][2 * jj + 1] = __float_as_int(rh1);
-#else
-                upk2(acc_finish2(ah[0], ah[1]), rh0, rh1);
-                Sh[sl][2 * jj] = __float_as_int(__fmul_rn(rh0, r0));
-                Sh[sl][2 * jj + 1] = __float_as_int(__fmul_rn(rh1, r1));
-#endif
-            } else {
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const float hv = h[sl][2 * jj + i];
-                    const int acc = acc_init_t<FAST>(__fadd_rn(__fadd_rn(bri[i], __fmul_rn(dri[i], hv)), gin[i])) + Sg[sl][2 * jj + i];
-                    const float r = sigmoid_approx(acc_finish_t<FAST>(acc), rcp_r);
-                    const int acch = acc_init_t<FAST>(__fadd_rn(bhi[i], __fmul_rn(dhi[i], hv))) + Sh[sl][2 * jj + i];
-                    Sh[sl][2 * jj + i] = __float_as_int(__fmul_rn(acc_finish_t<FAST>(acch), r));
-                }
+            for (int i = 0; i < 2; i++) {
+                const float hv = h[sl][2 * jj + i];
+                const int acc = acc_init_t<FAST>(__fadd_rn(__fadd_rn(bri[i], __fmul_rn(dri[i], hv)), gin[i])) + Sg[sl][2 * jj + i];
+                const float r = sigmoid_approx(acc_finish_t<FAST>(acc), rcp);
+                const int acch = acc_init_t<FAST>(__fadd_rn(bhi[i], __fmul_rn(dhi[i], hv))) + Sh[sl][2 * jj + i];
+                Sh[sl][2 * jj + i] = __float_as_int(__fmul_rn(acc_finish_t<FAST>(acch), r));
             }
         }
     }
@@ -513,31 +314,10 @@ __device__ __forceinline__ void activations(const ComputeCtx &C, float (&h)[GPW]
         for (int jj = 0; jj < 2; jj++) {
             const float2 gv = *reinterpret_cast<const float2 *>(tile_z + 8 * jj * GIN_ROW + C.gcol[sl]);
             const float gin[2] = {gv.x, gv.y};
-            if constexpr (FAST) {
-                int a[2];
-#if LPCNET_PACK_ACT
-                {
-                    float a0, a1;
-                    upk2(add2(mul2(add2(add2(mul2(pk2(dz.x, dz.y), pk2(h[sl][2 * jj], h[sl][2 * jj + 1])), pk2(bz.x, bz.y)), pk2(gv.x, gv.y)), k2(LPCNET_SCALE)), k2(LPCNET_CVT_MAGIC)), a0, a1);
-                    a[0] = __float_as_int(a0) + Sg[sl][2 * jj]; a[1] = __float_as_int(a1) + Sg[sl][2 * jj + 1];
-                }
-#else
 #pragma unroll
-                for (int i = 0; i < 2; i++)
-                    a[i] = acc_init_t<true>(__fadd_rn(__fadd_rn(bzi[i], __fmul_rn(dzi[i], h[sl][2 * jj + i])), gin[i])) + Sg[sl][2 * jj + i];
-#endif
-                f32x2 num, den;
-                rational2(acc_finish2(a[0], a[1]), LPCNET_SIGMOID_COEF, num, den);
-                float n0, n1, d0, d1;
-                upk2(num, n0, n1); upk2(den, d0, d1);
-                Sg[sl][2 * jj] = __float_as_int(fmaxf(0.f, fminf(1.f, __fmaf_rn(n0, rcp_emul(d0, rcp_z), 0.5f))));
-                Sg[sl][2 * jj + 1] = __float_as_int(fmaxf(0.f, fminf(1.f, __fmaf_rn(n1, rcp_emul(d1, rcp_z), 0.5f))));
-            } else {
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const int acc = acc_init_t<FAST>(__fadd_rn(__fadd_rn(bzi[i], __fmul_rn(dzi[i], h[sl][2 * jj + i])), gin[i])) + Sg[sl][2 * jj + i];
-                    Sg[sl][2 * jj + i] = __float_as_int(sigmoid_approx(acc_finish_t<FAST>(acc), rcp_z));
-                }
+            for (int i = 0; i < 2; i++) {
+                const int acc = acc_init_t<FAST>(__fadd_rn(__fadd_rn(bzi[i], __fmul_rn(dzi[i], h[sl][2 * jj + i])), gin[i])) + Sg[sl][2 * jj + i];
+                Sg[sl][2 * jj + i] = __float_as_int(sigmoid_approx(acc_finish_t<FAST>(acc), rcp));
             }
         }
     }
@@ -551,41 +331,13 @@ __device__ __forceinline__ void activations(const ComputeCtx &C, float (&h)[GPW]
             const float2 gv = *reinterpret_cast<const float2 *>(tile_h + 8 * jj * GIN_ROW + C.gcol[sl]);
             const float gin[2] = {gv.x, gv.y};
             uint32_t q[2];
-            if constexpr (FAST) {
-                f32x2 num, den;
-                rational2(add2(pk2(__int_as_float(Sh[sl][2 * jj]), __int_as_float(Sh[sl][2 * jj + 1])), pk2(gin[0], gin[1])), LPCNET_TANH_COEF, num, den);
-                float d0, d1, t0, t1;
-                upk2(den, d0, d1);
-                upk2(mul2(num, pk2(rcp_emul(d0, rcp_h), rcp_emul(d1, rcp_h))), t0, t1);
-                const float hh[2] = {fmaxf(-1.f, fminf(1.f, t0)), fmaxf(-1.f, fminf(1.f, t1))};
-                float hn[2];
-#if LPCNET_PACK_ACT
-                {
-                    const f32x2 z2 = pk2(__int_as_float(Sg[sl][2 * jj]), __int_as_float(Sg[sl][2 * jj + 1]));
-                    upk2(add2(mul2(z2, pk2(h[sl][2 * jj], h[sl][2 * jj + 1])), mul2(one_minus2(z2), pk2(hh[0], hh[1]))), hn[0], hn[1]);
-                    h[sl][2 * jj] = hn[0]; h[sl][2 * jj + 1] = hn[1];
-                }
-#else
 #pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const float z = __int_as_float(Sg[sl][2 * jj + i]);
-                    hn[i] = __fadd_rn(__fmul_rn(z, h[sl][2 * jj + i]), __fmul_rn(__fsub_rn(1.f, z), hh[i]));
-                    h[sl][2 * jj + i] = hn[i];
-                }
-#endif
-                // quantised bytes in the low bytes of the biased patterns: fma -> add, safe to pack
-                float q0, q1;
-                upk2(add2(fma2(pk2(hn[0], hn[1]), k2(127.f), k2(127.f)), k2(LPCNET_CVT_MAGIC)), q0, q1);
-                q[0] = __float_as_uint(q0); q[1] = __float_as_uint(q1);
-            } else {
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const float hh = tanh_approx(__fadd_rn(__int_as_float(Sh[sl][2 * jj + i]), gin[i]), rcp_h);
-                    const float z = __int_as_float(Sg[sl][2 * jj + i]);
-                    const float hn = __fadd_rn(__fmul_rn(z, h[sl][2 * jj + i]), __fmul_rn(__fsub_rn(1.f, z), hh));
-                    h[sl][2 * jj + i] = hn;
-                    q[i] = quant_u8_t<FAST>(hn);
-                }
+            for (int i = 0; i < 2; i++) {
+                const float hh = tanh_approx(__fadd_rn(__int_as_float(Sh[sl][2 * jj + i]), gin[i]), rcp);
+                const float z = __int_as_float(Sg[sl][2 * jj + i]);
+                const float hn = __fadd_rn(__fmul_rn(z, h[sl][2 * jj + i]), __fmul_rn(__fsub_rn(1.f, z), hh));
+                h[sl][2 * jj + i] = hn;
+                q[i] = quant_u8_t<FAST>(hn);
             }
             // other buffer: readers of the old state are unaffected
             *reinterpret_cast<uint16_t *>(xs_nxt + (C.xoff[sl] ^ (H << 6)) + 4 * jj) = (uint16_t)__byte_perm(q[0], q[1], 0x0040);
@@ -601,15 +353,9 @@ __device__ __forceinline__ void grub(const ComputeCtx &C, const SampleParams &P,
     const int gid = C.gid, t = C.t, lane = C.lane, warp = C.warp;
     const RcpShared rcp = C.rcp;
     const int nxt = cur ^ 1;
-    const uint32_t xs_cur = C.xs0 + cur * XS_BYTES, lc = C.gid8 | (H << 6);
-    uint8_t *xs_nxt = smem + SM_XS + nxt * XS_BYTES;
-    const uint32_t kr = k0, kz = k0 + 1, kh = k0 + 2;
-    const float *tile_r = reinterpret_cast<const float *>(smem + SM_TILES + (kr & 3) * TILE_BYTES) + gid * GIN_ROW;
-    const float *tile_z = reinterpret_cast<const float *>(smem + SM_TILES + (kz & 3) * TILE_BYTES) + gid * GIN_ROW;
+    const uint32_t lc = C.gid8 | (H << 6), kh = k0 + 2;
     uint8_t *tile_hb = smem + SM_TILES + (kh & 3) * TILE_BYTES;
-    const float *tile_h = reinterpret_cast<const float *>(tile_hb) + gid * GIN_ROW;
-    const uint32_t mb_full = smem_u32(smem + MB_FULL), mb_empty = smem_u32(smem + MB_EMPTY);
-    (void)t; (void)warp; (void)rcp; (void)nxt; (void)xs_cur; (void)lc; (void)xs_nxt; (void)tile_r; (void)tile_z; (void)tile_h; (void)mb_full; (void)mb_empty; (void)lane;
+    const uint32_t mb_empty = smem_u32(smem + MB_EMPTY);
     mbar_wait(smem_u32(smem + MB_X) + 8 * H, par);               // new quantised GRU_A state complete; candidate-gate tile dead: GRU_B scratch may use it
     TRACEC(P, trstep, 27, warp == 0 ? lane : 1);
     // ---------------- GRU_B input GEMV (48 x 384 int8, block-sparse lists, dense or not): warp = (row group, K part) ----------------
@@ -683,19 +429,11 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
     if (threadIdx.x == 0) {
         mbar_init(bar, 1);
         for (int b = 0; b < NTILE; b++) { mbar_init(smem_u32(smem + MB_FULL) + 8 * b, NWP * ARRIVALS_PER_WARP); mbar_init(smem_u32(smem + MB_EMPTY) + 8 * b, NWC * ARRIVALS_PER_WARP); }
-        for (int b = 0; b < NTILE; b++) mbar_init(smem_u32(smem + MB_COND) + 8 * b, 1);
         for (int hh = 0; hh < 2; hh++) { mbar_init(smem_u32(smem + MB_IDX) + 8 * hh, ARRIVALS_PER_WARP); mbar_init(smem_u32(smem + MB_X) + 8 * hh, NWC * ARRIVALS_PER_WARP); mbar_init(smem_u32(smem + MB_ACCB) + 8 * hh, NWB * ARRIVALS_PER_WARP); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(bar, L.image_bytes);
-        const uint32_t CH = 16384;
-        for (uint32_t o = 0; o < L.image_bytes; o += CH) {
-            const uint32_t nbytes = min(CH, L.image_bytes - o);
-            bulk_g2s(smem_u32(smem + SM_IMAGE + o), P.image + o, nbytes, bar);
-        }
-    }
+    if (threadIdx.x == 0) stage_image(smem_u32(smem + SM_IMAGE), P.image, L.image_bytes, bar);
     const RcpShared rcp = {smem_u32(smem + SM_IMAGE + IM_RCP)};
     if (threadIdx.x == 0 && (rcp.addr & 0x1FFFu) != 0) __trap();      // the table-address trick of rcp_emul needs the 8 KB alignment
     int *idx_s = reinterpret_cast<int *>(smem + SM_IDX);
@@ -774,29 +512,17 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
                 int Sh[GPW][4], Sg[GPW][4];                              // candidate-gate sums (later rec_h * r) / r-gate, then z-gate sums (later z)
                 const int tl = warp == 0 ? lane : 1; (void)tl;    // (lane selector of the TRACE stamps)
                 TRACEC(P, step, 0, tl); TRACEW(P, step, 0);
-#if LPCNET_GRUB_FIRST & 2
                 if (step > 0) grub<1, FAST>(C, P, hb[1], k - 3, (step - 1) & 1, f_prev, s_fin[1], (step - 1) & 1);
                 TRACEC(P, step, 1, tl); TRACEW(P, step, 1);
                 gemv_rh<0>(C, Sh, Sg, step & 1);
-#else
-                gemv_rh<0>(C, Sh, Sg, step & 1);
-                TRACEC(P, step, 1, tl); TRACEW(P, step, 1);
-                if (step > 0) grub<1, FAST>(C, P, hb[1], k - 3, (step - 1) & 1, f_prev, s_fin[1], (step - 1) & 1);
-#endif
                 TRACEC(P, step, 2, tl); TRACEW(P, step, 2);       // = HB of half B (previous sample) signalled
                 mbar_wait(smem_u32(smem + MB_FULL) + 8 * (k & 3), (k >> 2) & 1);
                 TRACEC(P, step, 3, tl); TRACEW(P, step, 3);       // r tile of half A present
                 activations<0, FAST>(C, h[0], Sh, Sg, k, step & 1);
                 TRACEC(P, step, 4, tl); TRACEW(P, step, 4);
-#if LPCNET_GRUB_FIRST & 1
                 grub<0, FAST>(C, P, hb[0], k, step & 1, f, s_fin[0], step & 1, step);
                 TRACEC(P, step, 5, tl); TRACEW(P, step, 5);
                 gemv_rh<1>(C, Sh, Sg, step & 1);
-#else
-                gemv_rh<1>(C, Sh, Sg, step & 1);
-                TRACEC(P, step, 5, tl); TRACEW(P, step, 5);
-                grub<0, FAST>(C, P, hb[0], k, step & 1, f, s_fin[0], step & 1, step);
-#endif
                 TRACEC(P, step, 6, tl); TRACEW(P, step, 6);       // = HB of half A signalled
                 mbar_wait(smem_u32(smem + MB_FULL) + 8 * ((k + 3) & 3), ((k + 3) >> 2) & 1);
                 TRACEC(P, step, 7, tl); TRACEW(P, step, 7);       // r tile of half B present
@@ -828,55 +554,19 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
         const int p = warp - NWC;
         const uint32_t mb_full = smem_u32(smem + MB_FULL), mb_empty = smem_u32(smem + MB_EMPTY), mb_idx = smem_u32(smem + MB_IDX);
         uint32_t k = 0, it = 0;
-#if LPCNET_COND_TMA
-        const uint32_t mb_cond = smem_u32(smem + MB_COND);
-        int nlive[2] = {0, 0};                                           // live tile rows of the halves (the live slots of a half are its first rows)
-        for (int hh = 0; hh < 2; hh++)
-            for (int si = 0; si < HALF; si++) { bool live; slot_stream<ONE>(cta_s0, hh, si, spc, n, live); nlive[hh] += live ? 1 : 0; }
-#endif
         for (int f = 0; f < P.nframes; f++) {
             const float *condA_f = P.condA + (size_t)f * n * (3 * GIN_ROW);
             for (int t_ = 0; t_ < spf; t_++, it++)
 #pragma unroll 1
                 for (int hh = 0; hh < (one ? 1 : 2); hh++) {
-#if LPCNET_COND_TMA
-                    const int nl = nlive[hh];
-                    if (p == 0) {
-                        // conditioning rows of the half-step's three tiles, ahead of the indices (gather_half_tma).  A slot is written only
-                        // after every compute warp has released its previous contents; the r tile takes the slot whose last rows hold the
-                        // half's GRU_B state scratch, which the sampler reads until it publishes the indices: those rows are left out here.
-#pragma unroll 1
-                        for (int gi = 0; gi < 3; gi++) {
-                            const uint32_t kk = k + gi;
-                            const int gate = gi == 0 ? 1 : (gi == 1 ? 0 : 2), rows = gi == 0 ? min(nl, LATE_ROW0) : nl;
-                            mbar_wait(mb_empty + 8 * (kk & 3), ((kk >> 2) & 1) ^ 1);
-                            if (lane == 0) {
-                                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic accesses of the old contents before the async-proxy writes
-                                mbar_expect_tx(mb_cond + 8 * (kk & 3), (uint32_t)rows * (GIN_ROW * 4));
-                                if (rows > 0) {                                              // the rows of a half are consecutive streams: ONE bulk copy, pitch = tile pitch
-                                    bool live;
-                                    const int sg0 = slot_stream<ONE>(cta_s0, hh, 0, spc, n, live);
-                                    bulk_g2s(smem_u32(smem + SM_TILES + (kk & 3) * TILE_BYTES), cond_row(condA_f, n, gate, sg0), (uint32_t)rows * (GIN_ROW * 4), mb_cond + 8 * (kk & 3));
-                                }
-                            }
-                            __syncwarp();
-                        }
-                    }
-#endif
                     mbar_wait(mb_idx + 8 * hh, it & 1);                  // indices of this sample of the half are in idx_s
                     TRACE(P, (int)it, 10 + 4 * hh, p == 0 ? lane : 1);
 #pragma unroll 1
                     for (int gi = 0; gi < 3; gi++, k++) {
                         const int gate = gi == 0 ? 1 : (gi == 1 ? 0 : 2);    // fill order r, z, h
-#if LPCNET_COND_TMA
-                        mbar_wait(mb_cond + 8 * (k & 3), (k >> 2) & 1);      // conditioning rows landed (issued after the slot was released)
-                        gather_half_tma<ONE>(reinterpret_cast<float *>(smem + SM_TILES + (k & 3) * TILE_BYTES), condA_f, n, cta_s0, hh, spc, nl, gi == 0 ? LATE_ROW0 : HALF,
-                                    P.emb_sig, P.emb_pred, P.emb_exc, idx_s + hh * 3 * HALF, gate, p, lane);
-#else
                         mbar_wait(mb_empty + 8 * (k & 3), ((k >> 2) & 1) ^ 1);  // previous contents of the tile consumed
                         gather_half<ONE>(reinterpret_cast<float *>(smem + SM_TILES + (k & 3) * TILE_BYTES), condA_f, n, cta_s0, hh, spc,
                                     P.emb_sig, P.emb_pred, P.emb_exc, idx_s + hh * 3 * HALF, gate, p, lane);
-#endif
                         warp_arrive(mb_full + 8 * (k & 3), lane);
                         TRACE(P, (int)it, 11 + 4 * hh + gi, p == 0 ? lane : 1);
                     }
@@ -951,36 +641,8 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
 #pragma unroll
                 for (int j = 0; j < NB; j++) hbv[j] = hBs[j * HALF + si];
                 int val = 0;
-#if LPCNET_EXPERIMENT == 1
-                { const long long t0 = clock64(); while (clock64() - t0 < 1000) { } }      // (timing experiment: a slower sampler)
-#endif
-#if LPCNET_TREE_PAR
-                // The nodes of the first three tree levels (1..7, rows always in shared memory) do not depend on any decision: all seven are
-                // evaluated side by side (seven independent 16-term chains interleave in the pipeline) and the three decisions are then just
-                // compares, instead of three strictly serial load -> chain -> tanh -> shuffle -> compare rounds on the sample's critical path.
-                {
-                    float totn[8];
 #pragma unroll
-                    for (int nd = 1; nd < 8; nd++) {
-                        const float *wr = fcw + nd * FCW_ROW;
-                        const float4 a0 = *reinterpret_cast<const float4 *>(wr), a1 = *reinterpret_cast<const float4 *>(wr + 4);
-                        const float4 a2 = *reinterpret_cast<const float4 *>(wr + 8), a3 = *reinterpret_cast<const float4 *>(wr + 12);
-                        const float w16[16] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w, a3.x, a3.y, a3.z, a3.w};
-                        float sum = wr[2 * NB - ch * NB + ch];
-                        const float fac = wr[2 * NB - ch * NB + 2 + ch];
-#pragma unroll
-                        for (int j = 0; j < NB; j++) sum = __fadd_rn(sum, __fmul_rn(w16[j], hbv[j]));
-                        const float mine = __fmul_rn(fac, tanh_approx(sum, rcp));
-                        totn[nd] = __fadd_rn(mine, __shfl_xor_sync(0xffffffffu, mine, 16));
-                    }
-                    val = thr[0] < totn[1] ? 1 : 0;
-                    val = (val << 1) | (thr[1] < (val ? totn[3] : totn[2]) ? 1 : 0);
-                    const float t3 = (val & 2) ? ((val & 1) ? totn[7] : totn[6]) : ((val & 1) ? totn[5] : totn[4]);
-                    val = (val << 1) | (thr[2] < t3 ? 1 : 0);
-                }
-#endif
-#pragma unroll
-                for (int b = (LPCNET_TREE_PAR ? 3 : 0); b < (LPCNET_EXPERIMENT == 2 ? 6 : 8); b++) {                            // sample_mdense, nnet.c:186-211
+                for (int b = 0; b < 8; b++) {                               // sample_mdense, nnet.c:186-211
                     const int i = (1 << b) | val;
                     // this lane's channel: a sequential 16-term chain
                     float w16[16], sum, fac;
@@ -1004,21 +666,6 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
                     const float other = __shfl_xor_sync(0xffffffffu, mine, 16);
                     const float tot = __fadd_rn(mine, other);            // channel 0 + channel 1 (commutative: both lanes get the same bits)
                     val = (val << 1) | (thr[b] < tot ? 1 : 0);
-#if LPCNET_FCW_PREFETCH
-                    // The node of level b+2 is one of two adjacent rows (288 bytes) once this decision is known.  If that level's rows are not in
-                    // shared memory, start them towards L1 now: an L2 round trip (~1 k cycles under load, twice per sample) leaves the serial
-                    // chain indices -> tiles -> GRU -> sampler -> indices.
-                    if (b + 2 < 8 && ch == 0) {
-                        const int i2 = (1 << (b + 2)) | (val << 1);
-                        if (!(b + 2 < 3 || (b + 2 < 6 && i2 + 1 < fcw_nodes))) {
-                            const char *r2 = reinterpret_cast<const char *>(P.fcw + (size_t)i2 * FCW_ROW);
-                            asm volatile("prefetch.global.L1 [%0];" ::"l"(r2));
-                            asm volatile("prefetch.global.L1 [%0];" ::"l"(r2 + 128));
-                            asm volatile("prefetch.global.L1 [%0];" ::"l"(r2 + 256));
-                            asm volatile("prefetch.global.L1 [%0];" ::"l"(r2 + 2 * FCW_ROW * 4 - 4));
-                        }
-                    }
-#endif
                 }
                 int exc = val;
                 float pcm;

@@ -17,8 +17,7 @@
 #ifndef LPCNET_NA
 #define LPCNET_NA 384          // GRU_A units this translation unit is compiled for
 #endif
-#include "engine.h"
-#include "devmath.cuh"
+#include "sample_common.cuh"
 
 namespace lpcnet_b200 {
 namespace LPCNET_KNS {
@@ -28,20 +27,6 @@ namespace {
 constexpr int F_THREADS = (F_NWC + 1) * 32;
 
 enum { FB_IDX = 1, FB_READ = 2, FB_X = 3, FB_ACCB = 4, FB_HB = 5 };
-
-__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
-{
-    asm volatile("{\n.reg .pred p;\nFWAIT_LOOP:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra FWAIT_DONE;\nbra FWAIT_LOOP;\nFWAIT_DONE:\n}\n" ::"r"(bar), "r"(parity) : "memory");
-}
 
 // 8 gathered conditioning inputs of one (gate, neuron group) for this lane's stream: ((cond + E_sig[a]) + E_pred[b]) + E_exc[c]
 __device__ __forceinline__ void gather8(float g[8], const float *__restrict__ c, const float *__restrict__ e0,
@@ -93,11 +78,7 @@ __global__ void __launch_bounds__(F_THREADS, 1) lpcnet_sample_kernel_f32(const _
     const uint32_t bar = smem_u32(smem + F_MBAR);
     if (threadIdx.x == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
     __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(bar, L.image_bytes);
-        const uint32_t CH = 16384;
-        for (uint32_t o = 0; o < L.image_bytes; o += CH) bulk_g2s(smem_u32(smem + F_IMAGE + o), P.image + o, min(CH, L.image_bytes - o), bar);
-    }
+    if (threadIdx.x == 0) stage_image(smem_u32(smem + F_IMAGE), P.image, L.image_bytes, bar);
     const uint16_t *rcp = reinterpret_cast<const uint16_t *>(smem + F_IMAGE + FI_RCP);
     float *xs = reinterpret_cast<float *>(smem + F_XS);
     float *hBs = reinterpret_cast<float *>(smem + F_HB);          // [2][16][32]

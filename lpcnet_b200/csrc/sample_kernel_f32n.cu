@@ -16,8 +16,7 @@
 #ifndef LPCNET_NA
 #define LPCNET_NA 384          // GRU_A units this translation unit is compiled for
 #endif
-#include "engine.h"
-#include "devmath.cuh"
+#include "sample_common.cuh"
 
 namespace lpcnet_b200 {
 namespace LPCNET_KNS {
@@ -26,20 +25,6 @@ namespace {
 
 enum { NB_IDX = 1, NB_X = 2, NB_ACCB = 3, NB_HB = 4 };
 constexpr int CNT_ALL = FN_THREADS, CNT_CMP = FN_NWC * 32;
-
-__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
-{
-    asm volatile("{\n.reg .pred p;\nNWAIT_LOOP:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra NWAIT_DONE;\nbra NWAIT_LOOP;\nNWAIT_DONE:\n}\n" ::"r"(bar), "r"(parity) : "memory");
-}
 
 // y[s] = fma(w[c], x[s][pos + c], y[s]), c = 0..3, for the blocks of this lane's row, in list order (one row of
 // sparse_sgemv_accum8x4 / sgemv_accum8x4, float).  `nb` is this lane's list length, `nbmax` the longest list in the warp
@@ -101,11 +86,7 @@ __device__ __forceinline__ void run(const SampleParams &P, uint8_t *smem)
     const uint32_t bar = smem_u32(smem + FN_MBAR);
     if (threadIdx.x == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
     __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(bar, L.image_bytes);
-        const uint32_t CH = 16384;
-        for (uint32_t o = 0; o < L.image_bytes; o += CH) bulk_g2s(smem_u32(smem + FN_IMAGE + o), P.image + o, min(CH, L.image_bytes - o), bar);
-    }
+    if (threadIdx.x == 0) stage_image(smem_u32(smem + FN_IMAGE), P.image, L.image_bytes, bar);
     const uint16_t *rcp = reinterpret_cast<const uint16_t *>(smem + FN_IMAGE + FNI_RCP);
     float *xs = reinterpret_cast<float *>(smem + FN_X);            // [2][FN_S][NA]
     float *hBs = reinterpret_cast<float *>(smem + FN_HB);          // [2][NB][FN_S]
