@@ -88,12 +88,15 @@ LPCNET_EXPORT LPCNetB200Batch *lpcnet_b200_batch_create_ex(int n_streams, const 
 LPCNET_EXPORT void lpcnet_b200_batch_destroy(LPCNetB200Batch *b);
 /* GRU_A units and the switches in effect. */
 LPCNET_EXPORT int lpcnet_b200_batch_model_info(const LPCNetB200Batch *b, int *gru_a_units, LPCNetB200Config *cfg);
-/* lpcnet_reset() (reference src/lpcnet.c:174) applied to every stream. */
+/* lpcnet_reset() (reference src/lpcnet.c:174) applied to every stream.  It also clears the decoder memory (the previous
+ * superframe's cepstrum, LPCNetDecState.vq_mem), as lpcnet_decoder_init() does to a loaded state: a reset stream starts a new
+ * utterance. */
 LPCNET_EXPORT int lpcnet_b200_batch_reset(LPCNetB200Batch *b);
-/* lpcnet_reset() for the listed streams only: they start a new utterance (two silent frames, fresh RNG) while the other
- * streams of the batch carry on.  Every stream has its own frame counter. */
+/* lpcnet_reset() for the listed streams only: they start a new utterance (two silent frames, fresh RNG, decoder memory
+ * cleared as above) while the other streams of the batch carry on.  Every stream has its own frame counter. */
 LPCNET_EXPORT int lpcnet_b200_batch_reset_streams(LPCNetB200Batch *b, const int *streams, int count);
-/* lpcnet_reset_signal() (reference src/lpcnet.c:226-233, used by the PLC): clears the sample-rate state only. */
+/* lpcnet_reset_signal() (reference src/lpcnet.c:226-233, used by the PLC): clears the sample-rate state only; the 100 Hz state
+ * and the decoder memory stay. */
 LPCNET_EXPORT int lpcnet_b200_batch_reset_signal(LPCNetB200Batch *b);
 LPCNET_EXPORT int lpcnet_b200_batch_streams(const LPCNetB200Batch *b);
 
@@ -202,14 +205,18 @@ LPCNET_EXPORT void lpcnet_b200_stream_destroy(void *stream);
 LPCNET_EXPORT int lpcnet_b200_stream_sync(void *stream);
 
 /* == lpcnet_decode() per stream, `npackets` times ==
- * packets: [n_streams][npackets][8] bytes ; pcm: [n_streams][npackets*640] int16 */
+ * packets: [n_streams][npackets][8] bytes ; pcm: [n_streams][npackets*640] int16
+ * Decode and synthesis share one per-stream state, as lpcnet_decode() drives the LPCNetState inside LPCNetDecState: a decode
+ * advances the frame counter by 4 per packet and leaves its last frame's conditioning for _synthesize_tail, and the decoder
+ * memory carries from call to call (and through _export_state / _import_state and snapshots). */
 LPCNET_EXPORT int lpcnet_b200_batch_decode(LPCNetB200Batch *b, const unsigned char *packets, int npackets, short *pcm);
 LPCNET_EXPORT int lpcnet_b200_batch_decode_device(LPCNetB200Batch *b, const unsigned char *d_packets, int npackets,
                                                   short *d_pcm, void *cuda_stream);
 
 /* == the analysis side, batched (SURVEY 8f N2): feature extraction and the 1.6 kb/s encoder ==
  * n independent LPCNetEncState streams (reference src/lpcnet_private.h:55-75) on one device, all starting from
- * lpcnet_encoder_create() (zeroed state, src/lpcnet_enc.c:471-482).  Results equal the reference's per-stream calls. */
+ * lpcnet_encoder_create() (zeroed state, src/lpcnet_enc.c:471-482).  Results equal the reference's per-stream calls.
+ * As with a synthesis batch, consecutive `_device` calls may use different CUDA streams and may be mixed with host calls. */
 typedef struct LPCNetB200EncBatch LPCNetB200EncBatch;
 LPCNET_EXPORT LPCNetB200EncBatch *lpcnet_b200_enc_create(int n_streams, int device);
 LPCNET_EXPORT void lpcnet_b200_enc_destroy(LPCNetB200EncBatch *e);

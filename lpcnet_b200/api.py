@@ -349,6 +349,16 @@ class EncBatch:
             raise LPCNetB200Error("lpcnet_b200_enc_encode: " + _err())
         return out
 
+    def compute_features_device(self, d_pcm_ptr, nframes, d_features_ptr, cuda_stream=None):
+        """d_pcm [n][nframes*160] int16 -> d_features [n][nframes][36] float32, both device pointers."""
+        if self._L.lpcnet_b200_enc_compute_features_device(self._h, d_pcm_ptr, int(nframes), d_features_ptr, cuda_stream) != 0:
+            raise LPCNetB200Error("lpcnet_b200_enc_compute_features_device: " + _err())
+
+    def encode_device(self, d_pcm_ptr, npackets, d_packets_ptr, cuda_stream=None):
+        """d_pcm [n][npackets*640] int16 -> d_packets [n][npackets][8] uint8, both device pointers."""
+        if self._L.lpcnet_b200_enc_encode_device(self._h, d_pcm_ptr, int(npackets), d_packets_ptr, cuda_stream) != 0:
+            raise LPCNetB200Error("lpcnet_b200_enc_encode_device: " + _err())
+
     def compute_features4(self, pcm):
         """pcm [n][P*640] int16 -> features [n][P*4][36] (lpcnet_compute_features: superframe analysis without quantisation)."""
         p = np.ascontiguousarray(pcm, dtype=np.int16)
@@ -470,8 +480,13 @@ class Batch:
         if self._L.lpcnet_b200_batch_set_pcm_sink(self._h, d_ptr, int(pitch_samples), int(first_row)) != 0:
             raise LPCNetB200Error(_err())
 
-    def synthesize_device(self, d_features_ptr, nframes, stride, d_pcm_ptr, samples_per_frame=160, cuda_stream=None):
-        r = self._L.lpcnet_b200_batch_synthesize_device(self._h, d_features_ptr, nframes, stride, samples_per_frame, d_pcm_ptr, cuda_stream)
+    def synthesize_device(self, d_features_ptr, nframes, stride, d_pcm_ptr, samples_per_frame=160, cuda_stream=None, preload=0):
+        """Device pointers in and out.  preload > 0: the first `preload` samples of every stream's row of d_pcm hold the forced
+        signal of the first frame (lpcnet_b200_batch_synthesize_device_ex)."""
+        if preload:
+            r = self._L.lpcnet_b200_batch_synthesize_device_ex(self._h, d_features_ptr, nframes, stride, samples_per_frame, d_pcm_ptr, int(preload), cuda_stream)
+        else:
+            r = self._L.lpcnet_b200_batch_synthesize_device(self._h, d_features_ptr, nframes, stride, samples_per_frame, d_pcm_ptr, cuda_stream)
         if r != 0:
             raise LPCNetB200Error("lpcnet_b200_batch_synthesize_device: " + _err())
 

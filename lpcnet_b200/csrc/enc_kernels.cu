@@ -631,9 +631,25 @@ struct LPCNetB200EncBatch {
     void *d_in; size_t d_in_cap;
     void *d_out; size_t d_out_cap;
     cudaStream_t stream;
+    // Ordering of the encoder state across CUDA streams, as in LPCNetB200Batch: every call that enqueues work records `order_ev`
+    // on the stream it used and the next call makes ITS stream wait for that event first, so consecutive `_device` calls may
+    // use different streams and may be mixed with the host-pointer calls.
+    cudaEvent_t order_ev; cudaStream_t last_stream; bool has_order;
 };
 
 namespace lpcnet_b200 { void build_fft_tables(std::vector<float> &dct, std::vector<float> &tw, std::vector<int16_t> &br); }
+
+static int enc_order_enter(LPCNetB200EncBatch *e, cudaStream_t st)
+{
+    if (e->has_order && e->last_stream != st) CK(cudaStreamWaitEvent(st, e->order_ev, 0));
+    return 0;
+}
+static int enc_order_leave(LPCNetB200EncBatch *e, cudaStream_t st)
+{
+    CK(cudaEventRecord(e->order_ev, st));
+    e->last_stream = st; e->has_order = true;
+    return 0;
+}
 
 static int enc_grow(void **p, size_t *cap, size_t bytes)
 {
@@ -653,6 +669,7 @@ void lpcnet_b200_enc_destroy(LPCNetB200EncBatch *e)
     cudaSetDevice(e->device);
     if (e->stream) cudaStreamSynchronize(e->stream);
     void *ptrs[] = {e->state, e->half_window, e->dct, e->twiddles, e->pitch_pow, e->cb, e->bitrev, e->d_in, e->d_out};
+    if (e->order_ev) { if (e->has_order) cudaEventSynchronize(e->order_ev); cudaEventDestroy(e->order_ev); }
     for (void *p : ptrs) if (p) cudaFree(p);
     if (e->stream) cudaStreamDestroy(e->stream);
     free(e);
@@ -662,7 +679,9 @@ int lpcnet_b200_enc_reset(LPCNetB200EncBatch *e)
 {
     if (!e) { set_error("null encoder batch"); return -1; }
     CK(cudaSetDevice(e->device));
+    if (enc_order_enter(e, e->stream)) return -1;
     CK(cudaMemsetAsync(e->state, 0, sizeof(EncState) * (size_t)e->n, e->stream));    // lpcnet_encoder_init: memset(st, 0) (lpcnet_enc.c:471-475)
+    if (enc_order_leave(e, e->stream)) return -1;
     CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
@@ -699,6 +718,7 @@ LPCNetB200EncBatch *lpcnet_b200_enc_create(int n_streams, int device)
     up((void **)&e->twiddles, tw.data(), tw.size() * 4); up((void **)&e->bitrev, br.data(), br.size() * 2); up((void **)&e->pitch_pow, pp.data(), pp.size() * 4);
     if (ok && cudaMalloc((void **)&e->state, sizeof(EncState) * (size_t)n_streams) != cudaSuccess) ok = false;
     if (ok && cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) ok = false;
+    if (ok && cudaEventCreateWithFlags(&e->order_ev, cudaEventDisableTiming) != cudaSuccess) ok = false;
     if (!ok || lpcnet_b200_enc_reset(e) != 0) { set_error("encoder batch: device allocation failed: %s", cudaGetErrorString(cudaGetLastError())); lpcnet_b200_enc_destroy(e); return nullptr; }
     return e;
 }
@@ -723,11 +743,12 @@ static int enc_run_device(LPCNetB200EncBatch *e, int mode, const short *d_pcm16,
     if (mode == 1 && !e->cb) { set_error("encode: no VQ codebooks loaded (lpcnet_b200_enc_set_codebooks)"); return -1; }
     EncArgs a{e->state, e->n, d_pcm16, d_pcmf, units, d_features, d_packets,
               EncTables{e->half_window, e->dct, reinterpret_cast<const c32 *>(e->twiddles), e->bitrev, e->pitch_pow, e->cb}};
+    if (enc_order_enter(e, st)) return -1;
     if (mode == 0) enc_kernel<0><<<e->n, ENC_THREADS, 0, st>>>(a);
     else if (mode == 1) enc_kernel<1><<<e->n, ENC_THREADS, 0, st>>>(a);
     else enc_kernel<2><<<e->n, ENC_THREADS, 0, st>>>(a);
     CK(cudaGetLastError());
-    return 0;
+    return enc_order_leave(e, st);
 }
 
 static int enc_run_host(LPCNetB200EncBatch *e, int mode, const void *pcm, bool is_float, int units, float *features, unsigned char *packets)

@@ -119,6 +119,25 @@ void ref_frame_network_deferred(void *st, const float *features) { run_frame_net
 void ref_frame_network_flush(void *st) { run_frame_network_flush((LPCNetState *)st); }
 void ref_reset_signal(void *st) { lpcnet_reset_signal((LPCNetState *)st); }
 
+/* ---- the decoder's state (LPCNetDecState, lpcnet_private.h:50-53) on an explicit handle.  It starts with its LPCNetState, so
+ * the entry points above also take a decoder handle. ---- */
+void *ref_dec_state_create(const unsigned char *blob, int len)
+{
+    LPCNetDecState *st = lpcnet_decoder_create();
+    if (lpcnet_load_model((LPCNetState *)st, blob, len) != 0) { lpcnet_decoder_destroy(st); return NULL; }
+    return st;
+}
+void ref_dec_state_destroy(void *st) { lpcnet_decoder_destroy((LPCNetDecState *)st); }
+int ref_decode(void *st, const unsigned char *packet, short *pcm) { return lpcnet_decode((LPCNetDecState *)st, packet, pcm); }
+/* what lpcnet_decoder_init does to a loaded state: lpcnet_reset, and the previous superframe's cepstrum cleared */
+void ref_dec_reset(void *st)
+{
+    LPCNetDecState *d = (LPCNetDecState *)st;
+    lpcnet_reset(&d->lpcnet_state);
+    memset(d->vq_mem, 0, sizeof(d->vq_mem));
+}
+void ref_dec_state_copy(void *dst, const void *src) { *(LPCNetDecState *)dst = *(const LPCNetDecState *)src; }
+
 /* ---- encoder / feature extraction (SURVEY 8f N2): the reference's own entry points on one stream with a fresh state ---- */
 /* lpcnet_compute_single_frame_features (lpcnet_enc.c:919) per 160-sample frame: pcm [nframes*160] -> features [nframes][36] */
 int ref_features_stream(const short *pcm, int nframes, float *features)

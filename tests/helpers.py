@@ -146,13 +146,13 @@ def oracle_synth(features, kind="int8", nthreads=8, tag="", model_blob=None):
     return pcm
 
 
-def oracle_decode(packets, kind="int8", nthreads=8, model_blob=None):
-    """packets [n][P][8] uint8 -> pcm [n][P*640] int16 (with `model_blob` when given)."""
+def oracle_decode(packets, kind="int8", nthreads=8, model_blob=None, tag=""):
+    """packets [n][P][8] uint8 -> pcm [n][P*640] int16 (of the variant `tag`, or of `model_blob` when given)."""
     L = oracle_lib()
     p = np.ascontiguousarray(packets, dtype=np.uint8)
     n, P, _ = p.shape
     pcm = np.zeros((n, P * 640), dtype=np.int16)
-    L.oracle_decode_batch(oracle_model(kind, "", model_blob), p.ctypes.data, n, P, nthreads, pcm.ctypes.data)
+    L.oracle_decode_batch(oracle_model(kind, tag, model_blob), p.ctypes.data, n, P, nthreads, pcm.ctypes.data)
     return pcm
 
 
@@ -194,6 +194,13 @@ def ref_lib(build="A", tag=""):
                    ("ref_frame_network_flush", [c_p]), ("ref_reset_signal", [c_p])):
         getattr(L, fn).argtypes = at
         getattr(L, fn).restype = None
+    if hasattr(L, "ref_dec_state_create"):      # decoder-state entry points (ref_shim.c)
+        L.ref_dec_state_create.restype = c_p
+        L.ref_dec_state_create.argtypes = [ctypes.c_char_p, ctypes.c_int]
+        L.ref_decode.argtypes = [c_p, c_p, c_p]
+        for fn, at in (("ref_dec_state_destroy", [c_p]), ("ref_dec_reset", [c_p]), ("ref_dec_state_copy", [c_p, c_p])):
+            getattr(L, fn).argtypes = at
+            getattr(L, fn).restype = None
     return L
 
 
@@ -229,13 +236,20 @@ def digest(a):
     return "%s%s:%s" % (a.dtype.str, list(a.shape), hashlib.sha256(a.tobytes()).hexdigest())
 
 
-def ref_digest(key, compute):
+def ref_has(build, tag, *symbols):
+    """The reference of (build, tag) is compiled and exports the shim entry points `symbols` (a reference compiled before
+    oracle/ref_shim.c had them lacks them)."""
+    return have_ref(build, tag) and all(hasattr(ref_lib(build, tag), s) for s in symbols)
+
+
+def ref_digest(key, compute, runnable=True):
     """Digest of what the compiled reference returns for the input named `key` (compute() runs it).  Where the reference is
-    compiled it is run and must reproduce the digest stored in tests/golden/ref_digests.json (LPCNET_WRITE_REF_DIGESTS=1
-    stores it instead); elsewhere the stored digest stands in for the run."""
+    compiled (and `runnable`: it has what compute() calls, see ref_has) it is run and must reproduce the digest stored in
+    tests/golden/ref_digests.json (LPCNET_WRITE_REF_DIGESTS=1 stores it instead); elsewhere the stored digest stands in for
+    the run."""
     import json
     stored = json.load(open(REF_DIGESTS)) if os.path.exists(REF_DIGESTS) else {}
-    if not have_ref("A"):
+    if not have_ref("A") or not runnable:
         assert key in stored, "no stored reference digest for %s" % key
         return stored[key]
     d = digest(compute())
