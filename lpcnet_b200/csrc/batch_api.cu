@@ -439,6 +439,7 @@ void lpcnet_b200_batch_destroy(LPCNetB200Batch *b)
 {
     if (!b) return;
     cudaSetDevice(b->device);
+    if (b->order_ev && b->has_order) cudaEventSynchronize(b->order_ev);     // the last call's work may sit on a caller stream
     if (b->stream) cudaStreamSynchronize(b->stream);
     if (b->fs.side) { cudaStreamSynchronize(b->fs.side); cudaStreamDestroy(b->fs.side); }
     if (b->fs.ev_fork) cudaEventDestroy(b->fs.ev_fork);
@@ -455,7 +456,7 @@ void lpcnet_b200_batch_destroy(LPCNetB200Batch *b)
     model_free(&b->model);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
-    if (b->order_ev) { if (b->has_order) cudaEventSynchronize(b->order_ev); cudaEventDestroy(b->order_ev); }
+    if (b->order_ev) cudaEventDestroy(b->order_ev);
     if (b->stream) cudaStreamDestroy(b->stream);
     free(b);
 }
@@ -477,7 +478,11 @@ int lpcnet_b200_batch_set_codebooks(LPCNetB200Batch *b, const float *cb, size_t 
     if (!cb || n_floats != want) { set_error("codebooks: expected %zu floats", want); return -1; }
     CK(cudaSetDevice(b->device));
     if (!b->model.codebooks) CK(cudaMalloc((void **)&b->model.codebooks, want * sizeof(float)));
-    CK(cudaMemcpy(b->model.codebooks, cb, want * sizeof(float), cudaMemcpyHostToDevice));
+    // ordered like any other call: a decode still queued on a caller stream reads the codebooks it was called with
+    if (order_enter(b, b->stream)) return -1;
+    CK(cudaMemcpyAsync(b->model.codebooks, cb, want * sizeof(float), cudaMemcpyHostToDevice, b->stream));
+    if (order_leave(b, b->stream)) return -1;
+    CK(cudaStreamSynchronize(b->stream));
     return 0;
 }
 
@@ -898,7 +903,8 @@ void *lpcnet_b200_device_alloc(size_t bytes)
     return p;
 }
 void lpcnet_b200_device_free(void *p) { if (p) cudaFree(p); }
-int lpcnet_b200_memcpy_h2d(void *dst, const void *src, size_t bytes) { CK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); return 0; }
+// (from pageable memory cudaMemcpy may return before the DMA has landed; the synchronise makes the data visible to work on any stream)
+int lpcnet_b200_memcpy_h2d(void *dst, const void *src, size_t bytes) { CK(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); CK(cudaStreamSynchronize(0)); return 0; }
 int lpcnet_b200_memcpy_d2h(void *dst, const void *src, size_t bytes) { CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost)); return 0; }
 int lpcnet_b200_set_device(int device) { CK(cudaSetDevice(device)); return 0; }
 // CUDA streams for callers without their own CUDA binding (the `cuda_stream` argument of the `_device` entry points)

@@ -716,6 +716,7 @@ LPCNetB200EncBatch *lpcnet_b200_enc_create(int n_streams, int device)
     auto up = [&](void **dst, const void *src, size_t bytes) { if (ok && (cudaMalloc(dst, bytes) != cudaSuccess || cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess)) ok = false; };
     up((void **)&e->half_window, hw.data(), hw.size() * 4); up((void **)&e->dct, dct2.data(), dct2.size() * 4);
     up((void **)&e->twiddles, tw.data(), tw.size() * 4); up((void **)&e->bitrev, br.data(), br.size() * 2); up((void **)&e->pitch_pow, pp.data(), pp.size() * 4);
+    if (ok && cudaStreamSynchronize(0) != cudaSuccess) ok = false;        // the DMA of a pageable cudaMemcpy may outlive the call (model.cu model_load)
     if (ok && cudaMalloc((void **)&e->state, sizeof(EncState) * (size_t)n_streams) != cudaSuccess) ok = false;
     if (ok && cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) ok = false;
     if (ok && cudaEventCreateWithFlags(&e->order_ev, cudaEventDisableTiming) != cudaSuccess) ok = false;
@@ -732,7 +733,11 @@ int lpcnet_b200_enc_set_codebooks(LPCNetB200EncBatch *e, const float *cb, size_t
     if (!cb || n_floats != want) { set_error("codebooks: expected %zu floats", want); return -1; }
     CK(cudaSetDevice(e->device));
     if (!e->cb) CK(cudaMalloc((void **)&e->cb, want * sizeof(float)));
-    CK(cudaMemcpy(e->cb, cb, want * sizeof(float), cudaMemcpyHostToDevice));
+    // ordered like any other call: an encode still queued on a caller stream reads the codebooks it was called with
+    if (enc_order_enter(e, e->stream)) return -1;
+    CK(cudaMemcpyAsync(e->cb, cb, want * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    if (enc_order_leave(e, e->stream)) return -1;
+    CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
 

@@ -603,6 +603,9 @@ int model_load(DeviceModel *m, const unsigned char *blob, int len, const ModelCo
         UP(pitch_pow, pp, 64)
     }
 #undef UP
+    // cudaMemcpy from pageable memory may return before its DMA has landed, and the engine's kernels run on non-blocking
+    // streams that do not wait for the default stream: finish the upload before any of them can read it
+    ok = ok && cudaStreamSynchronize(0) == cudaSuccess;
     if (!ok) { set_error("model: device allocation/copy failed: %s", cudaGetErrorString(cudaGetLastError())); model_free(m); return -1; }
 
     return 0;

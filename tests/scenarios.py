@@ -489,9 +489,10 @@ def run_streams(backend, lib, factory, feats, streams, script, pool=None):
     return out
 
 
-def run_engine_script(batch, feats, streams, script):
+def run_engine_script(batch, feats, streams, script, finish=None):
     """The same script on a lpcnet_b200.Batch of len(streams) streams (with codebooks for a decode script).  Returns PCM
-    [n][script_outputs]."""
+    [n][script_outputs].  `finish`, if given, runs after the last op and before the outputs are joined (a batch stand-in
+    whose synthesize / decode only enqueue device work fills the arrays they returned there)."""
     ops, signal = script[0], script[2]
     total = script_outputs(script)
     forced = np.stack([forced_pcm(signal, s, total) for s in streams])
@@ -530,4 +531,6 @@ def run_engine_script(batch, feats, streams, script):
             batch.import_state(op[2], batch.export_state(op[1]))
     if snap is not None:
         batch.free_snapshot(snap)
+    if finish is not None:
+        finish()
     return np.concatenate(out, axis=1)
