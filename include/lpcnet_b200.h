@@ -213,6 +213,41 @@ LPCNET_EXPORT int lpcnet_b200_batch_decode(LPCNetB200Batch *b, const unsigned ch
 LPCNET_EXPORT int lpcnet_b200_batch_decode_device(LPCNetB200Batch *b, const unsigned char *d_packets, int npackets,
                                                   short *d_pcm, void *cuda_stream);
 
+/* == groups: several batches of one model shape in one per-sample launch ==
+ * Several existing batches on ONE device with the same GRU_A size, all int8, each at most once (at most 16): their
+ * synthesize / decode calls run as one.  Each member runs its own frame network and its own silent-frame launches, then every
+ * member's remaining frames take ONE per-sample kernel launch that spreads all members' streams over the SMs together (no
+ * CTA holds streams of two members).  Group stream g = the streams of batches[0], then batches[1], ... in order (the sum of
+ * their sizes); features, packets and PCM are laid out as for a batch of that many streams.
+ * A group call leaves every member in exactly the state (PCM, recurrent state, RNG, frame counters, decoder memory, what a
+ * later _synthesize_tail reads) the member's own call would leave it in on its rows of the inputs, from any member state.
+ * The per-stream lifecycle calls (reset, tail, deferred / flush, export / import, snapshots, codebooks) stay on the members,
+ * which keep their own switches (FEATURES_DELAY, END2END, LPC_GAMMA) and sparsity patterns.  Group calls are ordered with
+ * the members' own calls like any other call, so `_device` group calls may be mixed with member calls on any stream.
+ * A member with a PCM sink set is refused.  The group does not own its members: destroy the group before any member.
+ * group_create returns NULL (message: lpcnet_b200_last_error) for members on different devices, with different GRU_A
+ * sizes, a float member, a member listed twice, or more than 16 members.  LPCNET_B200_STREAMS_PER_CTA is read at create. */
+typedef struct LPCNetB200Group LPCNetB200Group;
+LPCNET_EXPORT LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int count);
+LPCNET_EXPORT void lpcnet_b200_group_destroy(LPCNetB200Group *g);
+LPCNET_EXPORT int lpcnet_b200_group_streams(const LPCNetB200Group *g);
+/* features [sum n][nframes][feature_stride] -> pcm [sum n][nframes*samples_per_frame] */
+LPCNET_EXPORT int lpcnet_b200_group_synthesize(LPCNetB200Group *g, const float *features, int nframes, int feature_stride,
+                                               int samples_per_frame, short *pcm);
+LPCNET_EXPORT int lpcnet_b200_group_synthesize_device(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride,
+                                                      int samples_per_frame, short *d_pcm, void *cuda_stream);
+/* packets [sum n][npackets][8] -> pcm [sum n][npackets*640]; every member needs its codebooks */
+LPCNET_EXPORT int lpcnet_b200_group_decode(LPCNetB200Group *g, const unsigned char *packets, int npackets, short *pcm);
+LPCNET_EXPORT int lpcnet_b200_group_decode_device(LPCNetB200Group *g, const unsigned char *d_packets, int npackets, short *d_pcm,
+                                                  void *cuda_stream);
+/* Device time (ms) of the per-sample launches of the last group call: the fused launches and the members' silent-frame
+ * launches (the latter until a member's next own call); *launches = engine kernels that call launched. */
+LPCNET_EXPORT float lpcnet_b200_group_last_sample_kernel_ms(const LPCNetB200Group *g, int *launches);
+/* Test hook (host only, no CUDA): the launch plan for members of n[count] streams on `sms` SMs.  *spc = the smallest streams
+ * per CTA (1..32) for which sum ceil(n[k] / spc) <= sms, 32 if none; override_spc > 0 pins it (LPCNET_B200_STREAMS_PER_CTA).
+ * Member k takes ceil(n[k] / spc) consecutive CTAs; *ctas = their total.  spc <= 16 selects the half-A-only schedule. */
+LPCNET_EXPORT int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_spc, int *spc, int *ctas);
+
 /* == the analysis side, batched (SURVEY 8f N2): feature extraction and the 1.6 kb/s encoder ==
  * n independent LPCNetEncState streams (reference src/lpcnet_private.h:55-75) on one device, all starting from
  * lpcnet_encoder_create() (zeroed state, src/lpcnet_enc.c:471-482).  Results equal the reference's per-stream calls.

@@ -64,6 +64,18 @@ def lib():
     L.lpcnet_b200_batch_last_sample_kernel_ms.restype = ctypes.c_float
     L.lpcnet_b200_batch_last_sample_kernel_ms.argtypes = [c_p, c_p]
     L.lpcnet_b200_batch_algorithmic_bytes.argtypes = [c_p, c_p, c_p]
+    # groups of batches (one per-sample launch for several models of one shape)
+    L.lpcnet_b200_group_create.restype = c_p
+    L.lpcnet_b200_group_create.argtypes = [c_p, ctypes.c_int]
+    L.lpcnet_b200_group_destroy.argtypes = [c_p]
+    L.lpcnet_b200_group_streams.argtypes = [c_p]
+    L.lpcnet_b200_group_synthesize.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p]
+    L.lpcnet_b200_group_synthesize_device.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p]
+    L.lpcnet_b200_group_decode.argtypes = [c_p, c_p, ctypes.c_int, c_p]
+    L.lpcnet_b200_group_decode_device.argtypes = [c_p, c_p, ctypes.c_int, c_p, c_p]
+    L.lpcnet_b200_group_last_sample_kernel_ms.restype = ctypes.c_float
+    L.lpcnet_b200_group_last_sample_kernel_ms.argtypes = [c_p, c_p]
+    L.lpcnet_b200_debug_group_plan.argtypes = [c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p]
     L.lpcnet_b200_batch_is_float.argtypes = [c_p]
     L.lpcnet_b200_batch_get_state.argtypes = [c_p, ctypes.c_int, c_p, c_p, c_p, c_p, c_p]
     L.lpcnet_b200_debug_frame_network.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
@@ -561,6 +573,70 @@ class Batch:
         if self._L.lpcnet_b200_debug_tanh_x86(self._h, x.ctypes.data, a.ctypes.data, b.ctypes.data, int(x.size)) != 0:
             raise LPCNetB200Error(_err())
         return a, b
+
+
+def group_plan(sizes, sms, override_spc=0):
+    """Launch plan of a group whose members have `sizes` streams on `sms` SMs: (streams per CTA, CTA count)
+    (lpcnet_b200_debug_group_plan; host only, needs no GPU)."""
+    n = (ctypes.c_int * len(sizes))(*[int(v) for v in sizes])
+    spc, ctas = ctypes.c_int(0), ctypes.c_int(0)
+    if lib().lpcnet_b200_debug_group_plan(n, len(sizes), int(sms), int(override_spc), ctypes.byref(spc), ctypes.byref(ctas)) != 0:
+        raise LPCNetB200Error("debug_group_plan: " + _err())
+    return int(spc.value), int(ctas.value)
+
+
+class Group:
+    """The synthesize / decode calls of several int8 Batch objects of one GRU_A size on one device as one call: one per-sample
+    launch for all their streams (lpcnet_b200_group_*).  Group stream rows = batches[0]'s streams, then batches[1]'s, ...
+    The members stay usable on their own; the group keeps them alive and must be closed before they are."""
+
+    def __init__(self, batches):
+        self._L = lib()
+        self.batches = list(batches)
+        hs = (c_p * len(self.batches))(*[b._h for b in self.batches])
+        self._h = self._L.lpcnet_b200_group_create(hs, len(self.batches))
+        if not self._h:
+            raise LPCNetB200Error("lpcnet_b200_group_create: " + _err())
+        self.n = int(self._L.lpcnet_b200_group_streams(self._h))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.lpcnet_b200_group_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def synthesize(self, features, samples_per_frame=160):
+        """features [sum n][T][stride>=20] float32 (host) -> pcm [sum n][T*samples_per_frame] int16 (host)."""
+        f = np.ascontiguousarray(features, dtype=np.float32)
+        assert f.ndim == 3 and f.shape[0] == self.n
+        T, stride = f.shape[1], f.shape[2]
+        pcm = np.zeros((self.n, T * samples_per_frame), dtype=np.int16)
+        if self._L.lpcnet_b200_group_synthesize(self._h, f.ctypes.data, T, stride, samples_per_frame, pcm.ctypes.data) != 0:
+            raise LPCNetB200Error("lpcnet_b200_group_synthesize: " + _err())
+        return pcm
+
+    def synthesize_device(self, d_features_ptr, nframes, stride, d_pcm_ptr, samples_per_frame=160, cuda_stream=None):
+        if self._L.lpcnet_b200_group_synthesize_device(self._h, d_features_ptr, nframes, stride, samples_per_frame, d_pcm_ptr, cuda_stream) != 0:
+            raise LPCNetB200Error("lpcnet_b200_group_synthesize_device: " + _err())
+
+    def decode(self, packets):
+        """packets [sum n][P][8] uint8 -> pcm [sum n][P*640] int16."""
+        p = np.ascontiguousarray(packets, dtype=np.uint8)
+        assert p.ndim == 3 and p.shape[0] == self.n and p.shape[2] == 8
+        pcm = np.empty((self.n, p.shape[1] * 640), dtype=np.int16)
+        if self._L.lpcnet_b200_group_decode(self._h, p.ctypes.data, p.shape[1], pcm.ctypes.data) != 0:
+            raise LPCNetB200Error("lpcnet_b200_group_decode: " + _err())
+        return pcm
+
+    def decode_device(self, d_packets_ptr, npackets, d_pcm_ptr, cuda_stream=None):
+        if self._L.lpcnet_b200_group_decode_device(self._h, d_packets_ptr, npackets, d_pcm_ptr, cuda_stream) != 0:
+            raise LPCNetB200Error("lpcnet_b200_group_decode_device: " + _err())
+
+    def last_sample_kernel_ms(self):
+        k = ctypes.c_int(0)
+        ms = self._L.lpcnet_b200_group_last_sample_kernel_ms(self._h, ctypes.byref(k))
+        return float(ms), int(k.value)
 
 
 class LPCNet:

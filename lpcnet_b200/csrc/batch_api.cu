@@ -486,30 +486,57 @@ int lpcnet_b200_batch_set_codebooks(LPCNetB200Batch *b, const float *cb, size_t 
     return 0;
 }
 
-// launch the per-sample kernel for `nf` frames whose conditioning sits at chunk position `pos`
-static int launch_sample(LPCNetB200Batch *b, int pos, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st, bool time_it)
+// the per-sample kernel's parameters for `nf` frames of batch b whose conditioning sits at chunk position `pos`, except the
+// launch geometry and the rounding switch (spc, one_half, fast_cvt)
+static SampleParams sample_params(const LPCNetB200Batch *b, int pos, int nf, int spf, short *pcm, long long pcm_stride)
 {
-    const int n = b->n, na = b->model.na;
     SampleParams p = {};
     p.L = b->model.L; p.image = b->model.image;
     p.emb_sig = b->model.emb_sig; p.emb_pred = b->model.emb_pred; p.emb_exc = b->model.emb_exc; p.fcw = b->model.fcw;
-    p.spc = streams_per_cta_for(n, b->env_spc);
-    p.one_half = p.spc <= HALF && !b->env_two_halves;
-    p.fast_cvt = ((b->model.fast_cvt && !b->env_exact_cvt) ? 1 : 0) | (preload << 8);   // env LPCNET_B200_EXACT_CVT: force the conversion-unit path (tests)
-#ifdef LPCNET_TRACE
-    { static long long *d_trace = nullptr; if (!d_trace) { CK(cudaMalloc(&d_trace, (8 * 32 + 8 * 32 * 16) * 8)); CK(cudaMemset(d_trace, 0, (8 * 32 + 8 * 32 * 16) * 8)); } p.trace = d_trace; g_trace = d_trace; }
-#endif
     const CondFrame c = frame_at(b, pos);
     p.condA = c.A; p.condB = c.B; p.lpc_raw = c.L;
     p.gamma_pow = b->model.gamma_pow;
     p.hA = b->ss.hA; p.hB = b->ss.hB; p.last_sig = b->ss.last_sig; p.deemph = b->ss.deemph; p.last_exc = b->ss.last_exc; p.rng = b->ss.rng;
     p.pcm = pcm;
     p.pcm_stream_stride = pcm_stride;
-    p.n_streams = n; p.nframes = nf; p.spf = spf;
-    if (time_it) {      // event pair around the launch, resolved lazily by lpcnet_b200_batch_last_sample_kernel_ms (no sync here)
-        while ((int)b->kev->size() < b->kev_used + 2) { cudaEvent_t e; CK(cudaEventCreate(&e)); b->kev->push_back(e); }
-        CK(cudaEventRecord((*b->kev)[b->kev_used], st));
+    p.n_streams = b->n; p.nframes = nf; p.spf = spf;
+    return p;
+}
+// conversion-free rounding allowed for the batch's launches (env LPCNET_B200_EXACT_CVT: force the conversion-unit path, tests)
+static bool batch_fast_cvt(const LPCNetB200Batch *b) { return b->model.fast_cvt && !b->env_exact_cvt; }
+
+// an event pair around a per-sample launch, resolved lazily by lpcnet_b200_*_last_sample_kernel_ms (no sync here)
+static int time_launch(std::vector<cudaEvent_t> *kev, int *used, cudaStream_t st)
+{
+    while ((int)kev->size() < *used + 1) { cudaEvent_t e; CK(cudaEventCreate(&e)); kev->push_back(e); }
+    CK(cudaEventRecord((*kev)[*used], st));
+    ++*used;
+    return 0;
+}
+static float timed_ms(const std::vector<cudaEvent_t> *kev, int used)
+{
+    float total = 0.f;
+    for (int i = 0; i + 1 < used; i += 2) {
+        float ms = 0.f;
+        if (cudaEventSynchronize((*kev)[i + 1]) != cudaSuccess) return -1.f;
+        if (cudaEventElapsedTime(&ms, (*kev)[i], (*kev)[i + 1]) != cudaSuccess) return -1.f;
+        total += ms;
     }
+    return total;
+}
+
+// launch the per-sample kernel for `nf` frames whose conditioning sits at chunk position `pos`
+static int launch_sample(LPCNetB200Batch *b, int pos, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st, bool time_it)
+{
+    const int n = b->n, na = b->model.na;
+    SampleParams p = sample_params(b, pos, nf, spf, pcm, pcm_stride);
+    p.spc = streams_per_cta_for(n, b->env_spc);
+    p.one_half = p.spc <= HALF && !b->env_two_halves;
+    p.fast_cvt = (batch_fast_cvt(b) ? 1 : 0) | (preload << 8);
+#ifdef LPCNET_TRACE
+    { static long long *d_trace = nullptr; if (!d_trace) { CK(cudaMalloc(&d_trace, (8 * 32 + 8 * 32 * 16) * 8)); CK(cudaMemset(d_trace, 0, (8 * 32 + 8 * 32 * 16) * 8)); } p.trace = d_trace; g_trace = d_trace; }
+#endif
+    if (time_it && time_launch(b->kev, &b->kev_used, st)) return -1;
     const bool small_float = b->model.is_float && p.spc <= FN_S && !b->env_float_lane_stream;
     if (small_float) { p.L = b->model.Ln; p.image = b->model.image_n; }       // small batch: neuron-per-lane float kernel
     cudaError_t e;
@@ -521,14 +548,16 @@ static int launch_sample(LPCNetB200Batch *b, int pos, int nf, int spf, short *pc
     }
 #undef LPCNET_DISPATCH
     if (e != cudaSuccess) { set_error("per-sample kernel launch failed: %s", cudaGetErrorString(e)); return -1; }
-    if (time_it) { CK(cudaEventRecord((*b->kev)[b->kev_used + 1], st)); b->kev_used += 2; }
+    if (time_it && time_launch(b->kev, &b->kev_used, st)) return -1;
     return 0;
 }
 
 // The sample loops of the frames at chunk positions [pos0, pos0 + nf): per stream, frames whose post-increment frame
 // counter is <= FEATURES_DELAY are silent and do not advance the sample state (lpcnet.c:239-243).  b->fc = the streams'
-// counters before frame pos0 (host mirror), advanced here.  Returns the number of engine kernels launched, < 0 on error.
-static int sample_frames(LPCNetB200Batch *b, int pos0, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st)
+// counters before frame pos0 (host mirror).  sample_prefix handles the frames that are silent for at least one stream (zeros,
+// or one launch per frame with the still-silent streams put back) and returns in *live0 the first frame every stream runs;
+// frames [*live0, nf) then take one launch.  Returns the number of engine kernels launched, < 0 on error.
+static int sample_prefix(LPCNetB200Batch *b, int pos0, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st, int *live0)
 {
     const int n = b->n, delay = b->model.cfg.features_delay;
     int fc_min = 1 << 30, fc_max = 0;
@@ -553,6 +582,14 @@ static int sample_frames(LPCNetB200Batch *b, int pos0, int nf, int spf, short *p
             launches += 2;
         }
     }
+    *live0 = sil_any;
+    return launches;
+}
+static int sample_frames(LPCNetB200Batch *b, int pos0, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st)
+{
+    int sil_any = 0;
+    int launches = sample_prefix(b, pos0, nf, spf, pcm, pcm_stride, preload, st, &sil_any);
+    if (launches < 0) return -1;
     if (nf > sil_any) {
         if (launch_sample(b, pos0 + sil_any, nf - sil_any, spf, pcm + (size_t)sil_any * spf, pcm_stride, sil_any == 0 ? preload : 0, st, true)) return -1;
         launches += 1;
@@ -576,6 +613,15 @@ static int forward_to_sink(LPCNetB200Batch *b, const short *d_pcm, long long pcm
     return 0;
 }
 
+// The 100 Hz part of a chunk [c0, c0 + nf) of a call: the frame network on the batch's rows of the features; the chunk's last
+// frame is what a tail reads.  Returns the number of engine kernels launched.
+static int frame_chunk(LPCNetB200Batch *b, const float *d_feat, long long stream_stride, int frame_stride, int c0, int nf, cudaStream_t st)
+{
+    launch_frame_network(b->model, b->fs, d_feat + (size_t)c0 * frame_stride, stream_stride, frame_stride, b->n, nf, b->condA, b->condB, b->lpc_raw, st);
+    b->cond_last = nf - 1;
+    return frame_network_launches(b->model);
+}
+
 // Core: features and pcm are device pointers. `st` is the stream all work is enqueued on.
 static int synth_device(LPCNetB200Batch *b, const float *d_feat, long long stream_stride, int frame_stride, int nframes,
                         int spf, short *d_pcm, int preload, cudaStream_t st)
@@ -585,7 +631,6 @@ static int synth_device(LPCNetB200Batch *b, const float *d_feat, long long strea
     if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
     if (preload < 0 || preload > spf) { set_error("preload must be in 0..samples_per_frame"); return -1; }
     if (frame_stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
-    const int n = b->n;
     const long long pcm_stride = (long long)nframes * spf;
     if (b->sink && b->sink_pitch < pcm_stride) { set_error("PCM sink pitch %lld smaller than the call's %lld samples per stream", b->sink_pitch, pcm_stride); return -1; }
     int launches = 0;
@@ -593,9 +638,7 @@ static int synth_device(LPCNetB200Batch *b, const float *d_feat, long long strea
     if (order_enter(b, st)) return -1;
     for (int c0 = 0; c0 < nframes; c0 += CHUNK) {
         const int nf = nframes - c0 < CHUNK ? nframes - c0 : CHUNK;
-        launch_frame_network(b->model, b->fs, d_feat + (size_t)c0 * frame_stride, stream_stride, frame_stride, n, nf, b->condA, b->condB, b->lpc_raw, st);
-        launches += frame_network_launches(b->model);
-        b->cond_last = nf - 1;
+        launches += frame_chunk(b, d_feat, stream_stride, frame_stride, c0, nf, st);
         const int r = sample_frames(b, 0, nf, spf, d_pcm + (size_t)c0 * spf, pcm_stride, c0 == 0 ? preload : 0, st);
         if (r < 0) return -1;
         launches += r;
@@ -816,12 +859,297 @@ float lpcnet_b200_batch_last_sample_kernel_ms(const LPCNetB200Batch *b, int *lau
 {
     if (!b) return 0.f;
     if (launches) *launches = b->last_launches;
-    float total = 0.f;
-    for (int i = 0; i + 1 < b->kev_used; i += 2) {
-        float ms = 0.f;
-        if (cudaEventSynchronize((*b->kev)[i + 1]) != cudaSuccess) return -1.f;
-        if (cudaEventElapsedTime(&ms, (*b->kev)[i], (*b->kev)[i + 1]) != cudaSuccess) return -1.f;
-        total += ms;
+    return timed_ms(b->kev, b->kev_used);
+}
+
+// ---- groups: the synthesize / decode calls of several int8 batches of one GRU_A size on one device as one call ----
+// Each chunk runs every member's 100 Hz part and silent-frame prefix with the member's own launches, then ONE per-sample launch
+// for the frames that remain (GroupSampleParams, sample_kernel.cu).  The members keep all their state and host mirrors; the
+// group only holds the launch plan, a stream for its host-pointer calls and the event timers of its launches.
+struct LPCNetB200Group {
+    int count, device, na, n_total;
+    LPCNetB200Batch *m[GROUP_MAX];
+    int spc, ctas;                    // the launch plan (group_plan)
+    bool fast_cvt;                    // conversion-free rounding: only if every member allows it
+    uint32_t smem_bytes;              // largest shared-memory footprint of the members
+    cudaStream_t stream;
+    std::vector<cudaEvent_t> *kev;    // event pairs around the group's own per-sample launches of the last call
+    int kev_used, last_launches;
+};
+
+// One streams-per-CTA value for the whole launch: the smallest that puts every member on at most `sms` CTAs in total, member k
+// on ceil(n_k / spc) CTAs of its own; 32 when none does.  A one-member group plans as streams_per_cta_for.
+static int group_plan(const int *n, int count, int sms, int override_spc, int *ctas)
+{
+    auto total = [&](int spc) { int c = 0; for (int k = 0; k < count; k++) c += (n[k] + spc - 1) / spc; return c; };
+    int spc = STREAMS_PER_CTA;
+    if (override_spc > 0) spc = std::min(override_spc, STREAMS_PER_CTA);
+    else for (int s = 1; s <= STREAMS_PER_CTA; s++) if (total(s) <= sms) { spc = s; break; }
+    *ctas = total(spc);
+    return spc;
+}
+
+int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_spc, int *spc, int *ctas)
+{
+    if (!n || count < 1 || count > GROUP_MAX || sms < 1 || !spc || !ctas) { set_error("debug_group_plan: bad arguments"); return -1; }
+    for (int k = 0; k < count; k++) if (n[k] < 1) { set_error("debug_group_plan: member %d has no streams", k); return -1; }
+    *spc = group_plan(n, count, sms, override_spc, ctas);
+    return 0;
+}
+
+void lpcnet_b200_group_destroy(LPCNetB200Group *g)
+{
+    if (!g) return;
+    cudaSetDevice(g->device);
+    if (g->stream) { cudaStreamSynchronize(g->stream); cudaStreamDestroy(g->stream); }
+    if (g->kev) { for (cudaEvent_t e : *g->kev) cudaEventDestroy(e); delete g->kev; }
+    delete g;
+}
+
+LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int count)
+{
+    if (!batches || count < 1 || count > GROUP_MAX) { set_error("group_create: 1..%d member batches", GROUP_MAX); return nullptr; }
+    for (int k = 0; k < count; k++) {
+        const LPCNetB200Batch *b = batches[k];
+        if (!b) { set_error("group_create: member %d is NULL", k); return nullptr; }
+        if (b->model.is_float) { set_error("group_create: member %d holds a float model; groups run int8 models only", k); return nullptr; }
+        if (b->device != batches[0]->device) { set_error("group_create: member %d is on device %d, member 0 on device %d", k, b->device, batches[0]->device); return nullptr; }
+        if (b->model.na != batches[0]->model.na) { set_error("group_create: member %d has %d GRU_A units, member 0 has %d", k, b->model.na, batches[0]->model.na); return nullptr; }
+        for (int j = 0; j < k; j++) if (batches[j] == b) { set_error("group_create: member %d is listed twice (also member %d)", k, j); return nullptr; }
+    }
+    if (cudaSetDevice(batches[0]->device) != cudaSuccess) { set_error("group_create: cudaSetDevice(%d) failed", batches[0]->device); return nullptr; }
+    LPCNetB200Group *g = new LPCNetB200Group();
+    g->count = count; g->device = batches[0]->device; g->na = batches[0]->model.na;
+    g->fast_cvt = true;
+    int n[GROUP_MAX];
+    for (int k = 0; k < count; k++) {
+        LPCNetB200Batch *b = batches[k];
+        g->m[k] = b; n[k] = b->n; g->n_total += b->n;
+        g->fast_cvt = g->fast_cvt && batch_fast_cvt(b);
+        g->smem_bytes = std::max(g->smem_bytes, b->model.L.total_bytes);
+    }
+    int dev = g->device, sms = 0;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    const char *e = getenv("LPCNET_B200_STREAMS_PER_CTA");
+    g->spc = group_plan(n, count, sms, e ? atoi(e) : 0, &g->ctas);
+    g->kev = new std::vector<cudaEvent_t>();
+    if (cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) != cudaSuccess) {
+        set_error("group_create: cudaStreamCreate failed"); lpcnet_b200_group_destroy(g); return nullptr;
+    }
+    return g;
+}
+
+int lpcnet_b200_group_streams(const LPCNetB200Group *g) { return g ? g->n_total : 0; }
+
+// the fused launch over the members that still have frames [live0[k], nf) of the chunk to run
+static int launch_group(LPCNetB200Group *g, const int *live0, int nf, int spf, short *const *pcm, long long pcm_stride, cudaStream_t st)
+{
+    GroupSampleParams gp = {};
+    int ctas = 0;
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        if (live0[k] >= nf) continue;
+        SampleParams &p = gp.m[gp.count];
+        p = sample_params(b, live0[k], nf - live0[k], spf, pcm[k] + (size_t)live0[k] * spf, pcm_stride);
+        p.spc = g->spc;
+        p.one_half = g->spc <= HALF;
+        p.fast_cvt = g->fast_cvt ? 1 : 0;
+        gp.cta0[gp.count++] = ctas;
+        ctas += (b->n + g->spc - 1) / g->spc;
+    }
+    if (!gp.count) return 0;
+    if (time_launch(g->kev, &g->kev_used, st)) return -1;
+    cudaError_t e;
+    switch (g->na) {
+    case 128: e = na128::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st); break;
+    case 256: e = na256::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st); break;
+    default:  e = na384::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st); break;
+    }
+    if (e != cudaSuccess) { set_error("group per-sample kernel launch failed: %s", cudaGetErrorString(e)); return -1; }
+    if (time_launch(g->kev, &g->kev_used, st)) return -1;
+    return 1;
+}
+
+// Core of the group calls: member k reads features feat[k] ([n_k][nframes][frame_stride]) and writes pcm[k] ([n_k][nframes*spf]),
+// all device pointers, everything on `st`.  Per chunk: every member's frame network, every member's silent prefix, one launch.
+static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_stride, int nframes, int spf, short *const *pcm, cudaStream_t st)
+{
+    if (nframes <= 0) return 0;
+    if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
+    if (frame_stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
+    const long long stream_stride = (long long)nframes * frame_stride, pcm_stride = (long long)nframes * spf;
+    int launches = 0;
+    g->kev_used = 0;
+    for (int k = 0; k < g->count; k++) {
+        g->m[k]->kev_used = 0;
+        if (order_enter(g->m[k], st)) return -1;
+    }
+    for (int c0 = 0; c0 < nframes; c0 += CHUNK) {
+        const int nf = std::min(CHUNK, nframes - c0);
+        int live0[GROUP_MAX];
+        short *pc[GROUP_MAX];
+        for (int k = 0; k < g->count; k++) {
+            LPCNetB200Batch *b = g->m[k];
+            pc[k] = pcm[k] + (size_t)c0 * spf;
+            launches += frame_chunk(b, feat[k], stream_stride, frame_stride, c0, nf, st);
+            const int r = sample_prefix(b, 0, nf, spf, pc[k], pcm_stride, 0, st, &live0[k]);
+            if (r < 0) return -1;
+            launches += r;
+        }
+        const int r = launch_group(g, live0, nf, spf, pc, pcm_stride, st);
+        if (r < 0) return -1;
+        launches += r;
+        for (int k = 0; k < g->count; k++) for (int &v : *g->m[k]->fc) v = std::min(1000, v + nf);
+    }
+    CK(cudaGetLastError());
+    for (int k = 0; k < g->count; k++) if (order_leave(g->m[k], st)) return -1;
+    g->last_launches = launches;
+    return 0;
+}
+
+static int group_check(LPCNetB200Group *g)
+{
+    if (!g) { set_error("null group"); return -1; }
+    for (int k = 0; k < g->count; k++)
+        if (g->m[k]->sink) { set_error("group call: member %d has a PCM sink set; groups do not forward PCM to sinks", k); return -1; }
+    CK(cudaSetDevice(g->device));
+    return 0;
+}
+
+int lpcnet_b200_group_synthesize_device(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride,
+                                        int samples_per_frame, short *d_pcm, void *cuda_stream)
+{
+    if (group_check(g)) return -1;
+    if (nframes <= 0) return 0;
+    if (!d_features || !d_pcm) { set_error("null buffer"); return -1; }
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
+    const float *feat[GROUP_MAX]; short *pcm[GROUP_MAX];
+    size_t row = 0;
+    for (int k = 0; k < g->count; k++) {
+        feat[k] = d_features + row * nframes * feature_stride;
+        pcm[k] = d_pcm + row * nframes * samples_per_frame;
+        row += g->m[k]->n;
+    }
+    int r = group_synth(g, feat, feature_stride, nframes, samples_per_frame, pcm, st);
+    if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
+    return r;
+}
+
+int lpcnet_b200_group_synthesize(LPCNetB200Group *g, const float *features, int nframes, int feature_stride,
+                                 int samples_per_frame, short *pcm)
+{
+    if (group_check(g)) return -1;
+    if (nframes <= 0) return 0;
+    if (!features || !pcm) { set_error("null buffer"); return -1; }
+    const float *feat[GROUP_MAX]; short *dp[GROUP_MAX];
+    for (int k = 0; k < g->count; k++) {      // each member's rows go through the member's own staging buffers
+        LPCNetB200Batch *b = g->m[k];
+        if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * (size_t)b->n * nframes * feature_stride)) return -1;
+        if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, sizeof(short) * (size_t)b->n * nframes * samples_per_frame)) return -1;
+        feat[k] = b->d_features; dp[k] = b->d_pcm;
+    }
+    size_t row = 0;
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        if (order_enter(b, g->stream)) return -1;
+        CK(cudaMemcpyAsync(b->d_features, features + row * nframes * feature_stride, sizeof(float) * (size_t)b->n * nframes * feature_stride,
+                           cudaMemcpyHostToDevice, g->stream));
+        if (order_leave(b, g->stream)) return -1;
+        row += b->n;
+    }
+    if (group_synth(g, feat, feature_stride, nframes, samples_per_frame, dp, g->stream)) return -1;
+    row = 0;
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        CK(cudaMemcpyAsync(pcm + row * nframes * samples_per_frame, b->d_pcm, sizeof(short) * (size_t)b->n * nframes * samples_per_frame,
+                           cudaMemcpyDeviceToHost, g->stream));
+        row += b->n;
+    }
+    CK(cudaStreamSynchronize(g->stream));
+    return 0;
+}
+
+// decode: every member's packet decoder into the member's feature staging, then the group synthesis over those features
+static int group_decode(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, cudaStream_t st)
+{
+    const float *feat[GROUP_MAX];
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        if (!b->model.codebooks) { set_error("group decode: member %d has no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)", k); return -1; }
+        if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * (size_t)b->n * npackets * 4 * NB_FEAT)) return -1;
+        feat[k] = b->d_features;
+    }
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        if (order_enter(b, st)) return -1;
+        launch_decode_packets(b->model, b->fs, packets[k], b->n, npackets, b->d_features, st);
+        if (order_leave(b, st)) return -1;
+    }
+    if (group_synth(g, feat, NB_FEAT, npackets * 4, FRAME_SIZE, pcm, st)) return -1;
+    g->last_launches += g->count;
+    return 0;
+}
+
+int lpcnet_b200_group_decode_device(LPCNetB200Group *g, const unsigned char *d_packets, int npackets, short *d_pcm, void *cuda_stream)
+{
+    if (group_check(g)) return -1;
+    if (npackets <= 0) return 0;
+    if (!d_packets || !d_pcm) { set_error("null buffer"); return -1; }
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
+    const uint8_t *pk[GROUP_MAX]; short *pcm[GROUP_MAX];
+    size_t row = 0;
+    for (int k = 0; k < g->count; k++) {
+        pk[k] = d_packets + row * npackets * 8;
+        pcm[k] = d_pcm + row * npackets * 640;
+        row += g->m[k]->n;
+    }
+    int r = group_decode(g, pk, npackets, pcm, st);
+    if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
+    return r;
+}
+
+int lpcnet_b200_group_decode(LPCNetB200Group *g, const unsigned char *packets, int npackets, short *pcm)
+{
+    if (group_check(g)) return -1;
+    if (npackets <= 0) return 0;
+    if (!packets || !pcm) { set_error("null buffer"); return -1; }
+    const uint8_t *pk[GROUP_MAX]; short *dp[GROUP_MAX];
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        if (ensure(b, (void **)&b->d_packets, &b->d_packets_cap, (size_t)b->n * npackets * 8)) return -1;
+        if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, sizeof(short) * (size_t)b->n * npackets * 640)) return -1;
+        pk[k] = b->d_packets; dp[k] = b->d_pcm;
+    }
+    size_t row = 0;
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        if (order_enter(b, g->stream)) return -1;
+        CK(cudaMemcpyAsync(b->d_packets, packets + row * npackets * 8, (size_t)b->n * npackets * 8, cudaMemcpyHostToDevice, g->stream));
+        if (order_leave(b, g->stream)) return -1;
+        row += b->n;
+    }
+    if (group_decode(g, pk, npackets, dp, g->stream)) return -1;
+    row = 0;
+    for (int k = 0; k < g->count; k++) {
+        LPCNetB200Batch *b = g->m[k];
+        CK(cudaMemcpyAsync(pcm + row * npackets * 640, b->d_pcm, sizeof(short) * (size_t)b->n * npackets * 640, cudaMemcpyDeviceToHost, g->stream));
+        row += b->n;
+    }
+    CK(cudaStreamSynchronize(g->stream));
+    return 0;
+}
+
+// the group's fused launches plus the members' own launches for their silent-frame prefixes, in the last group call (the
+// latter until the member's next call)
+float lpcnet_b200_group_last_sample_kernel_ms(const LPCNetB200Group *g, int *launches)
+{
+    if (!g) return 0.f;
+    if (launches) *launches = g->last_launches;
+    if (cudaSetDevice(g->device) != cudaSuccess) return -1.f;
+    float total = timed_ms(g->kev, g->kev_used);
+    for (int k = 0; k < g->count && total >= 0.f; k++) {
+        const float ms = timed_ms(g->m[k]->kev, g->m[k]->kev_used);
+        total = ms < 0.f ? -1.f : total + ms;
     }
     return total;
 }

@@ -348,6 +348,17 @@ struct SampleParams {
 // (the layout of SampleParams is kept as it is: one more word made the int8 kernel slower; new per-call switches
 // are packed into existing words)
 
+// One per-sample launch over the batches of a group (lpcnet_b200_group_*, int8 only): member k's streams are CTAs
+// [cta0[k], cta0[k] + ceil(n_k / spc)) of the grid, every CTA holds streams of one member only.  spc, one_half and fast_cvt are
+// the group's and the same in every m[k].
+constexpr int GROUP_MAX = 16;        // members of a group: GROUP_MAX SampleParams fill most of the 4 KB of kernel parameters
+struct GroupSampleParams {
+    SampleParams m[GROUP_MAX];
+    int cta0[GROUP_MAX];
+    int count;
+};
+static_assert(sizeof(GroupSampleParams) <= 4096, "group launch parameters exceed the kernel parameter space");
+
 // gru_a_dense_feature output of one frame (the GRU_A conditioning rows).  int8 flavour: gate-major with the row pitch of a gather tile
 // (na + 8 floats): the producers' gather_half (sample_kernel.cu) reads the row of (gate, stream) at one offset, and the rows of a half's
 // consecutive streams for one gate are one contiguous piece of memory; float flavour: the reference's [stream][3*na].
@@ -382,7 +393,8 @@ void launch_decode_packets(const DeviceModel &m, const FrameState &fs, const uin
 #define LPCNET_DECLARE_LAUNCHERS(ns) namespace ns { \
     cudaError_t launch_sample_kernel(const SampleParams &p, cudaStream_t st); \
     cudaError_t launch_sample_kernel_f32(const SampleParams &p, cudaStream_t st); \
-    cudaError_t launch_sample_kernel_f32n(const SampleParams &p, cudaStream_t st);   /* p.L / p.image = DeviceModel::Ln / image_n, p.spc <= FN_S */ }
+    cudaError_t launch_sample_kernel_f32n(const SampleParams &p, cudaStream_t st);   /* p.L / p.image = DeviceModel::Ln / image_n, p.spc <= FN_S */ \
+    cudaError_t launch_group_sample_kernel(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st); }
 LPCNET_DECLARE_LAUNCHERS(na128)
 LPCNET_DECLARE_LAUNCHERS(na256)
 LPCNET_DECLARE_LAUNCHERS(na384)

@@ -412,8 +412,10 @@ __device__ __forceinline__ void grub(const ComputeCtx &C, const SampleParams &P,
 
 }  // namespace
 
+// The body of the per-sample kernel for the streams of `P` that CTA `cta` of their batch holds.  A single-batch launch runs it
+// with its own parameters and blockIdx.x; a group launch with the parameters of the CTA's member and the member-local CTA index.
 template <bool FAST, bool ONE>
-__global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const __grid_constant__ SampleParams P)
+__device__ __forceinline__ void sample_body(const SampleParams &P, int cta)
 {
     extern __shared__ __align__(128) uint8_t smem[];
     const SmemLayout &L = P.L;
@@ -421,7 +423,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
     const int n = P.n_streams;
     constexpr bool one = ONE;                                     // spc <= 16: half-A-only schedule (SampleParams::one_half)
     const int spc = P.spc;
-    const int cta_s0 = blockIdx.x * spc;
+    const int cta_s0 = cta * spc;
     const int spf = P.spf;
 
     // ---- mbarriers; stage the constant image with TMA bulk copies ----
@@ -698,6 +700,36 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const 
             P.rng[s] = rng.z; P.rng[(size_t)n + s] = rng.w; P.rng[2 * (size_t)n + s] = rng.jsr; P.rng[3 * (size_t)n + s] = rng.jcong;
         }
     }
+}
+
+template <bool FAST, bool ONE>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_sample_kernel(const __grid_constant__ SampleParams P)
+{
+    sample_body<FAST, ONE>(P, blockIdx.x);
+}
+
+// Several batches of one GRU_A size in one launch: member k holds CTAs [cta0[k], cta0[k+1]) (GroupSampleParams, engine.h).  The
+// member's parameters are read where they lie, in the kernel's parameter space: a copy to shared memory has no room, as every
+// byte in front of the image is taken and the image's place is fixed by the RCPPS table alignment.
+template <bool FAST, bool ONE>
+__global__ void __launch_bounds__(SAMPLE_THREADS, 1) lpcnet_group_sample_kernel(const __grid_constant__ GroupSampleParams G)
+{
+    const int c = blockIdx.x;
+    int k = 0;
+#pragma unroll 1
+    for (int j = 1; j < G.count; j++) if (c >= G.cta0[j]) k = j;
+    sample_body<FAST, ONE>(G.m[k], c - G.cta0[k]);
+}
+
+cudaError_t launch_group_sample_kernel(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st)
+{
+    const bool one = g.m[0].one_half != 0, fast = (g.m[0].fast_cvt & 1) != 0;      // (the same in every member: the group's plan)
+    auto kern = fast ? (one ? lpcnet_group_sample_kernel<true, true> : lpcnet_group_sample_kernel<true, false>)
+                     : (one ? lpcnet_group_sample_kernel<false, true> : lpcnet_group_sample_kernel<false, false>);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    kern<<<ctas, SAMPLE_THREADS, smem_bytes, st>>>(g);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_sample_kernel(const SampleParams &p, cudaStream_t st)
