@@ -153,6 +153,23 @@ LPCNET_EXPORT LPCNetB200Snapshot *lpcnet_b200_batch_snapshot_create(LPCNetB200Ba
 LPCNET_EXPORT void lpcnet_b200_batch_snapshot_destroy(LPCNetB200Snapshot *s);
 LPCNET_EXPORT int lpcnet_b200_batch_snapshot_save(LPCNetB200Batch *b, LPCNetB200Snapshot *s);
 LPCNET_EXPORT int lpcnet_b200_batch_snapshot_restore(LPCNetB200Batch *b, const LPCNetB200Snapshot *s);
+/* ... and whole streams from rows of one batch to rows of another (or the same) batch, on the device: compacting a batch whose
+ * sessions ended, rebalancing the shards of a multi-GPU job, cloning a stream.  For k < count: row dst_rows[k] of dst becomes,
+ * bit for bit, what row src_rows[k] of src was before the call.  Copied: everything the exported blob carries (GRU states, signal
+ * history, de-emphasis, last excitation, conv/LPC delay lines, decoder memory, RNG, frame counter), the stream's deferred frames
+ * and its row of the conditioning a tail reads.  The source is unchanged; src == dst is allowed and every read sees the state
+ * from before the call (a rotation of rows works); source rows may repeat (cloning); destination rows must be distinct.  Rows
+ * not listed are untouched, their queues and tail conditioning included.
+ * Tails: afterwards dst accepts _synthesize_tail only if it did before and src did too; otherwise it refuses tails until its next
+ * frame-network run, as after an import.  The copied rows land in dst's current tail frame.  A copied stream with more queued
+ * frames than dst's queue holds makes that queue longer at its old end, which the other streams never read.
+ * Both batches must have the same GRU_A size, flavour (int8 / float) and switches (FEATURES_DELAY, END2END, LPC_GAMMA); weights are
+ * not compared: a row copied between two models continues under dst's weights.  src and dst may be on different devices of this
+ * process (peer DMA when the devices allow it, staged by the driver otherwise).  The call waits for all work queued on either
+ * batch, on any CUDA stream, and returns when the copy is complete; later calls on either batch are ordered after it.
+ * Returns -1 (message: lpcnet_b200_last_error) and changes nothing for a NULL argument, count < 0, a row out of range, a repeated
+ * destination row or batches that do not match.  count == 0 does nothing and succeeds. */
+LPCNET_EXPORT int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LPCNetB200Batch *src, const int *src_rows, int count);
 
 /* == multi-GPU: PCM sink ==  Streams shard across GPUs with no data-path exchange (SURVEY.md 8e); the only transfer is the
  * gather of the PCM.  With a sink set, every synthesize/decode `_device` call also copies each finished chunk (<= 16 frames)

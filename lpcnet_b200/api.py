@@ -44,6 +44,7 @@ def lib():
     L.lpcnet_b200_batch_snapshot_destroy.argtypes = [c_p]
     L.lpcnet_b200_batch_snapshot_save.argtypes = [c_p, c_p]
     L.lpcnet_b200_batch_snapshot_restore.argtypes = [c_p, c_p]
+    L.lpcnet_b200_batch_copy_streams.argtypes = [c_p, c_p, c_p, c_p, ctypes.c_int]
     L.lpcnet_b200_batch_set_pcm_sink.argtypes = [c_p, c_p, ctypes.c_longlong, ctypes.c_longlong]
     L.lpcnet_b200_ipc_export.argtypes = [c_p, c_p]
     L.lpcnet_b200_ipc_open.restype = c_p
@@ -487,6 +488,16 @@ class Batch:
 
     def free_snapshot(self, snap):
         self._L.lpcnet_b200_batch_snapshot_destroy(snap)
+
+    def copy_streams(self, dst_rows, src_batch, src_rows):
+        """Row dst_rows[k] of this batch becomes what row src_rows[k] of src_batch (this batch allowed) was before the call: the whole
+        stream state, its deferred frames and its tail conditioning, copied on the device (lpcnet_b200_batch_copy_streams)."""
+        d = np.ascontiguousarray(dst_rows, dtype=np.int32)
+        s = np.ascontiguousarray(src_rows, dtype=np.int32)
+        if d.shape != s.shape:
+            raise LPCNetB200Error("copy_streams: %d destination rows for %d source rows" % (d.size, s.size))
+        if self._L.lpcnet_b200_batch_copy_streams(self._h, d.ctypes.data, src_batch._h, s.ctypes.data, int(d.size)) != 0:
+            raise LPCNetB200Error("copy_streams: " + _err())
 
     def set_pcm_sink(self, d_ptr, pitch_samples, first_row):
         if self._L.lpcnet_b200_batch_set_pcm_sink(self._h, d_ptr, int(pitch_samples), int(first_row)) != 0:

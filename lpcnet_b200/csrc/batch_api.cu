@@ -46,7 +46,7 @@ struct LPCNetB200Batch {
     float *d_features; size_t d_features_cap;     // staging for host-pointer calls / decoder output
     short *d_pcm; size_t d_pcm_cap;
     uint8_t *d_packets; size_t d_packets_cap;
-    float *d_state; size_t d_state_cap;           // staging for export/import of one stream's state
+    float *d_state; size_t d_state_cap;           // staging for export/import of one stream's state and for copies between batches
     // run_frame_network_deferred queue: [DEFER_MAX][n][20] on the host, deferred_fill frames long.  Stream s has queued the LAST
     // (*dfill)[s] <= deferred_fill of them (a reset or an import empties one stream's queue, lpcnet.c:174-182).
     std::vector<float> *deferred; int deferred_fill; std::vector<int> *dfill;
@@ -169,30 +169,51 @@ struct StateView {
     SampleState ss;
     FrameState fs;
 };
+// One frame of conditioning as the per-sample kernel reads it: condA (int8 [3 gates][n][na + 8], float [n][3*na]), condB [n][3*NB],
+// raw LPC [n][16]
+struct CondFrame { float *A, *B, *L; };
+
 // words of one stream's exported state: floats hA[na] hB[16] last_sig[16] deemph conv1[168] conv2[256] lpc_carry[2][16] vq_mem[18],
 // then ints last_exc, frame_count, rng[4]
 __host__ __device__ inline int state_words(int na) { return na + NB + LPC_ORDER + 1 + 2 * FRAME_IN + 2 * COND + 2 * LPC_ORDER + NB_BANDS + 6; }
+// words a copy between batches adds behind them: the stream's row of the frame a tail reads, condA[3*na] condB[3*NB] raw LPC[16]
+__host__ __device__ inline int tail_words(int na) { return 3 * na + 3 * NB + LPC_ORDER; }
 
-// dir 0: state of stream s -> buf, dir 1: buf -> state of stream s
-__global__ void state_pack_kernel(StateView v, int s, float *buf, int dir)
+// The by-value record of stream s, the one place that knows its layout: the exported words in the order above, then, if `tail`
+// is given, the stream's row of that conditioning frame (a_float: the float flavour's condA layout).  UNPACK: record -> stream.
+template <bool UNPACK>
+__device__ void move_record(const StateView &v, size_t s, float *rec, const CondFrame &tail, int a_float)
 {
     const size_t n = v.n;
     int o = 0;
     auto mv = [&](float *base, size_t stride, int count, size_t off) {
-        for (int i = threadIdx.x; i < count; i += blockDim.x) { float *p = base + off + (size_t)i * stride; if (dir) *p = buf[o + i]; else buf[o + i] = *p; }
+        for (int i = threadIdx.x; i < count; i += blockDim.x) { float *p = base + off + (size_t)i * stride; if (UNPACK) *p = rec[o + i]; else rec[o + i] = *p; }
         o += count;
     };
     mv(v.ss.hA, n, v.na, s); mv(v.ss.hB, n, NB, s); mv(v.ss.last_sig, n, LPC_ORDER, s); mv(v.ss.deemph, 1, 1, s);
-    mv(v.fs.conv1_state, 1, 2 * FRAME_IN, (size_t)s * 2 * FRAME_IN); mv(v.fs.conv2_state, 1, 2 * COND, (size_t)s * 2 * COND);
-    mv(v.fs.lpc_carry, 1, LPC_ORDER, (size_t)s * LPC_ORDER); mv(v.fs.lpc_carry, 1, LPC_ORDER, (n + s) * LPC_ORDER);
-    mv(v.fs.vq_mem, 1, NB_BANDS, (size_t)s * NB_BANDS);
+    mv(v.fs.conv1_state, 1, 2 * FRAME_IN, s * 2 * FRAME_IN); mv(v.fs.conv2_state, 1, 2 * COND, s * 2 * COND);
+    mv(v.fs.lpc_carry, 1, LPC_ORDER, s * LPC_ORDER); mv(v.fs.lpc_carry, 1, LPC_ORDER, (n + s) * LPC_ORDER);
+    mv(v.fs.vq_mem, 1, NB_BANDS, s * NB_BANDS);
     mv(reinterpret_cast<float *>(v.ss.last_exc), 1, 1, s); mv(reinterpret_cast<float *>(v.fs.frame_count), 1, 1, s);
     mv(reinterpret_cast<float *>(v.ss.rng), n, 4, s);
+    if (!tail.A) return;
+    const int na = v.na;
+    if (a_float) mv(tail.A, 1, 3 * na, s * 3 * na);
+    else for (int g = 0; g < 3; g++) mv(tail.A, 1, na, (g * n + s) * (na + 8));
+    mv(tail.B, 1, 3 * NB, s * 3 * NB);
+    mv(tail.L, 1, LPC_ORDER, s * LPC_ORDER);
 }
-
-// One frame of conditioning as the per-sample kernel reads it: condA (int8 [3 gates][n][na + 8], float [n][3*na]), condB [n][3*NB],
-// raw LPC [n][16]
-struct CondFrame { float *A, *B, *L; };
+// one block per record k of buf (`words` apart): stream rows[k] (rows == NULL: stream s0 + k)
+__global__ void streams_pack_kernel(StateView v, const int *rows, int s0, float *buf, int words, CondFrame tail, int a_float)
+{
+    const int k = blockIdx.x;
+    move_record<false>(v, rows ? rows[k] : s0 + k, buf + (size_t)k * words, tail, a_float);
+}
+__global__ void streams_unpack_kernel(StateView v, const int *rows, int s0, float *buf, int words, CondFrame tail, int a_float)
+{
+    const int k = blockIdx.x;
+    move_record<true>(v, rows ? rows[k] : s0 + k, buf + (size_t)k * words, tail, a_float);
+}
 
 // lpcnet_reset (lpcnet.c:174-182) for the listed streams (ids == NULL: all n streams); signal_only = lpcnet_reset_signal (lpcnet.c:226-233).
 // A full reset also zeroes the streams' entries of `tail` (the reference clears gru_a_condition, gru_b_condition and lpc), if given.
@@ -1283,9 +1304,15 @@ static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
     const size_t bytes = (size_t)state_words(b->model.na) * 4;
     if (ensure(b, (void **)&b->d_state, &b->d_state_cap, bytes)) return -1;
     if (order_enter(b, b->stream)) return -1;
-    if (dir) CK(cudaMemcpyAsync(b->d_state, buf, bytes, cudaMemcpyHostToDevice, b->stream));
-    state_pack_kernel<<<1, 128, 0, b->stream>>>(view_of(b), s, b->d_state, dir);
-    if (!dir) CK(cudaMemcpyAsync(buf, b->d_state, bytes, cudaMemcpyDeviceToHost, b->stream));
+    const int words = state_words(b->model.na);
+    const CondFrame none{nullptr, nullptr, nullptr};
+    if (dir) {
+        CK(cudaMemcpyAsync(b->d_state, buf, bytes, cudaMemcpyHostToDevice, b->stream));
+        streams_unpack_kernel<<<1, 128, 0, b->stream>>>(view_of(b), nullptr, s, b->d_state, words, none, 0);
+    } else {
+        streams_pack_kernel<<<1, 128, 0, b->stream>>>(view_of(b), nullptr, s, b->d_state, words, none, 0);
+        CK(cudaMemcpyAsync(buf, b->d_state, bytes, cudaMemcpyDeviceToHost, b->stream));
+    }
     if (order_leave(b, b->stream)) return -1;
     CK(cudaStreamSynchronize(b->stream));
     if (dir) {
@@ -1298,6 +1325,104 @@ static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
 }
 int lpcnet_b200_batch_export_state(LPCNetB200Batch *b, int s, void *buf) { return state_move(b, s, buf, 0); }
 int lpcnet_b200_batch_import_state(LPCNetB200Batch *b, int s, const void *buf) { return state_move(b, s, const_cast<void *>(buf), 1); }
+
+// ---- whole streams between batches on the device (compaction, shard rebalancing, cloning) ----
+// Each batch's staging buffer d_state holds [count] source rows, [count] destination rows, then the count records (move_record).
+// The records are packed on src's stream, copied into dst's staging (peer DMA across devices) and unpacked on dst's stream;
+// staging makes src == dst read every record before any is written.
+static int copy_check(const LPCNetB200Batch *dst, const int *dst_rows, const LPCNetB200Batch *src, const int *src_rows, int count)
+{
+    if (!dst || !dst_rows || !src || !src_rows || count < 0) { set_error("copy_streams: bad arguments"); return -1; }
+    if (dst->model.na != src->model.na) { set_error("copy_streams: dst has %d GRU_A units, src %d", dst->model.na, src->model.na); return -1; }
+    if (dst->model.is_float != src->model.is_float) { set_error("copy_streams: one batch holds an int8 model, the other a float model"); return -1; }
+    const ModelConfig &a = dst->model.cfg, &c = src->model.cfg;
+    if (a.features_delay != c.features_delay || a.end2end != c.end2end || a.lpc_gamma != c.lpc_gamma) {
+        set_error("copy_streams: model switches differ (FEATURES_DELAY %d / %d, END2END %d / %d, LPC_GAMMA %g / %g)",
+                  a.features_delay, c.features_delay, a.end2end, c.end2end, (double)a.lpc_gamma, (double)c.lpc_gamma);
+        return -1;
+    }
+    std::vector<char> seen(dst->n, 0);
+    for (int k = 0; k < count; k++) {
+        if (src_rows[k] < 0 || src_rows[k] >= src->n) { set_error("copy_streams: source row %d out of range (%d streams)", src_rows[k], src->n); return -1; }
+        if (dst_rows[k] < 0 || dst_rows[k] >= dst->n) { set_error("copy_streams: destination row %d out of range (%d streams)", dst_rows[k], dst->n); return -1; }
+        if (seen[dst_rows[k]]) { set_error("copy_streams: destination row %d listed twice", dst_rows[k]); return -1; }
+        seen[dst_rows[k]] = 1;
+    }
+    return 0;
+}
+
+int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LPCNetB200Batch *src, const int *src_rows, int count)
+{
+    if (copy_check(dst, dst_rows, src, src_rows, count)) return -1;
+    if (count == 0) return 0;
+    const int na = src->model.na, words = state_words(na) + tail_words(na), a_float = src->model.is_float;
+    const size_t rows_bytes = sizeof(int) * 2 * (size_t)count, bytes = rows_bytes + sizeof(float) * (size_t)count * words;
+    const bool tails = dst->cond_last >= 0 && src->cond_last >= 0;      // else dst refuses tails until its next frame-network run
+    const CondFrame none{nullptr, nullptr, nullptr};
+    std::vector<int> rows(2 * (size_t)count);
+    std::copy(src_rows, src_rows + count, rows.begin());
+    std::copy(dst_rows, dst_rows + count, rows.begin() + count);
+    CK(cudaSetDevice(src->device));
+    if (ensure(src, (void **)&src->d_state, &src->d_state_cap, bytes)) return -1;
+    CK(cudaSetDevice(dst->device));
+    if (ensure(dst, (void **)&dst->d_state, &dst->d_state_cap, bytes)) return -1;
+
+    // 1. pack on src's stream
+    CK(cudaSetDevice(src->device));
+    int *s_rows = reinterpret_cast<int *>(src->d_state);
+    float *s_rec = reinterpret_cast<float *>(reinterpret_cast<char *>(src->d_state) + rows_bytes);
+    if (order_enter(src, src->stream)) return -1;
+    CK(cudaMemcpyAsync(s_rows, rows.data(), rows_bytes, cudaMemcpyHostToDevice, src->stream));
+    streams_pack_kernel<<<count, 128, 0, src->stream>>>(view_of(src), s_rows, 0, s_rec, words, tails ? frame_at(src, src->cond_last) : none, a_float);
+    CK(cudaGetLastError());
+    // 2. src's order event marks the records ready; dst's stream waits for it (and for dst's own last call)
+    if (order_leave(src, src->stream)) return -1;
+    CK(cudaSetDevice(dst->device));
+    int *d_rows = reinterpret_cast<int *>(dst->d_state);
+    float *d_rec = reinterpret_cast<float *>(reinterpret_cast<char *>(dst->d_state) + rows_bytes);
+    if (order_enter(dst, dst->stream)) return -1;
+    if (dst != src) CK(cudaStreamWaitEvent(dst->stream, src->order_ev, 0));
+    // 3. into dst's staging
+    if (dst != src) {
+        CK(cudaMemcpyAsync(d_rows, rows.data(), rows_bytes, cudaMemcpyHostToDevice, dst->stream));
+        if (dst->device != src->device) CK(cudaMemcpyPeerAsync(d_rec, dst->device, s_rec, src->device, bytes - rows_bytes, dst->stream));
+        else CK(cudaMemcpyAsync(d_rec, s_rec, bytes - rows_bytes, cudaMemcpyDeviceToDevice, dst->stream));
+    }
+    // 4. unpack on dst's stream
+    streams_unpack_kernel<<<count, 128, 0, dst->stream>>>(view_of(dst), d_rows + count, 0, d_rec, words, tails ? frame_at(dst, dst->cond_last) : none, a_float);
+    CK(cudaGetLastError());
+    // 5. both orders end here; the call returns with the copy complete
+    if (order_leave(dst, dst->stream)) return -1;
+    CK(cudaStreamSynchronize(dst->stream));
+    CK(cudaSetDevice(src->device));
+    CK(cudaStreamSynchronize(src->stream));
+
+    // host mirrors: frame counters and deferred queues, read from src as it was before the call
+    const std::vector<int> sfc = *src->fc, sfill = *src->dfill;
+    const std::vector<float> sq = *src->deferred;
+    const int sF = src->deferred_fill;
+    int q_max = 0;
+    for (int k = 0; k < count; k++) q_max = std::max(q_max, sfill[src_rows[k]]);
+    const size_t sfr = (size_t)src->n * NB_FEAT, dfr = (size_t)dst->n * NB_FEAT;
+    if (q_max > dst->deferred_fill) {       // grow dst's queue at its old end: the other streams read only their last dfill frames
+        const int grow = q_max - dst->deferred_fill;
+        dst->deferred->resize(dfr * DEFER_MAX);
+        float *q = dst->deferred->data();
+        memmove(q + dfr * grow, q, sizeof(float) * dfr * dst->deferred_fill);
+        std::fill(q, q + dfr * grow, 0.f);
+        dst->deferred_fill = q_max;
+    }
+    const int dF = dst->deferred_fill;
+    for (int k = 0; k < count; k++) {
+        const int s = src_rows[k], d = dst_rows[k], qn = sfill[s];
+        for (int i = 0; i < qn; i++)
+            memcpy(dst->deferred->data() + dfr * (dF - qn + i) + (size_t)d * NB_FEAT, sq.data() + sfr * (sF - qn + i) + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
+        (*dst->dfill)[d] = qn;
+        (*dst->fc)[d] = sfc[s];
+    }
+    if (!tails) dst->cond_last = -1;
+    return 0;
+}
 
 // ---- whole-batch snapshot on the device (roll-back after speculative synthesis) ----
 // It also holds the frame a tail reads, as the reference's state copy holds gru_a_condition / gru_b_condition / lpc.
