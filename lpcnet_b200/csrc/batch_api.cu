@@ -29,17 +29,21 @@ static const int TAIL_SLOT = CHUNK;
 
 // the sample-rate part of the per-stream state (resettable part of struct LPCNetState), structure of arrays
 struct SampleState { float *hA, *hB, *last_sig, *deemph; int *last_exc; uint32_t *rng; };
+// One frame of conditioning as the per-sample kernel reads it: condA (int8 [3 gates][n][na + 8], float [n][3*na]), condB [n][3*NB],
+// raw LPC [n][16]
+struct CondFrame { float *A, *B, *L; };
+// device buffers of a copy of the per-stream state (a batch's shadow copy, a snapshot), for the parts it was allocated for
+struct StateCopy { SampleState ss; FrameState fs; CondFrame tail; };
 
 struct LPCNetB200Batch {
     int device, n;
     DeviceModel model;
     FrameState fs;
     SampleState ss;
-    SampleState shadow;                           // scratch copy for frames in which only SOME streams are still in their silent warm-up
-    int *d_nsil;                                  // [n] silent frames of each stream in the segment being processed (mixed segments only)
-    FrameState fshadow;                           // scratch copy of the 100 Hz state for flushes in which only SOME streams have queued frames
-    int *d_keep;                                  // [DEFER_MAX][n] 1 = the stream sits that queued frame out (such flushes only)
-    std::vector<int> *fc;                         // host mirror of fs.frame_count
+    StateCopy shadow;                             // scratch copy for calls in which only SOME streams advance: the sample-rate part for frames
+                                                  // some streams sit out in their silent warm-up, the 100 Hz part for flushes some have no frame for
+    int *d_mask;                                  // [DEFER_MAX][n] per frame of such a call: 1 = the stream sits the frame out
+    std::vector<int> fc;                          // host mirror of fs.frame_count
     // work buffers: CHUNK chunk slots + TAIL_SLOT
     float *condA, *condB, *lpc_raw;
     int cond_last;                                // slot of the conditioning a tail reads (a chunk position or TAIL_SLOT); -1 = none since an import
@@ -48,8 +52,8 @@ struct LPCNetB200Batch {
     uint8_t *d_packets; size_t d_packets_cap;
     float *d_state; size_t d_state_cap;           // staging for export/import of one stream's state and for copies between batches
     // run_frame_network_deferred queue: [DEFER_MAX][n][20] on the host, deferred_fill frames long.  Stream s has queued the LAST
-    // (*dfill)[s] <= deferred_fill of them (a reset or an import empties one stream's queue, lpcnet.c:174-182).
-    std::vector<float> *deferred; int deferred_fill; std::vector<int> *dfill;
+    // dfill[s] <= deferred_fill of them (a reset or an import empties one stream's queue, lpcnet.c:174-182).
+    std::vector<float> deferred; int deferred_fill; std::vector<int> dfill;
     cudaStream_t stream;
     // Ordering of the engine state across CUDA streams: every call that enqueues work records `order_ev` on the stream it
     // used; the next call makes ITS stream wait for that event first (and host-side readers synchronise on it).  A caller
@@ -58,7 +62,7 @@ struct LPCNetB200Batch {
     int env_spc;                                  // LPCNET_B200_STREAMS_PER_CTA (0: automatic)
     bool env_exact_cvt, env_float_lane_stream, env_two_halves;    // LPCNET_B200_EXACT_CVT / _FLOAT_LANE_STREAM / _TWO_HALVES, read once at create time (tests)
     cudaEvent_t ev0, ev1;                         // user timer (lpcnet_b200_batch_timer_*)
-    std::vector<cudaEvent_t> *kev;                // event pairs around every per-sample kernel launch of the last call
+    std::vector<cudaEvent_t> kev;                 // event pairs around every per-sample kernel launch of the last call
     int kev_used;
     int last_launches;
     // PCM sink (multi-GPU gather): after every chunk the chunk's PCM block is also copied, on a copy stream that overlaps the next
@@ -163,117 +167,92 @@ static void kiss99_seed(uint32_t st[4])
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// per-stream state kernels (rare paths: resets, export / import, mixed silent segments) — plain strided copies
-struct StateView {
-    int n, na;
-    SampleState ss;
-    FrameState fs;
-};
-// One frame of conditioning as the per-sample kernel reads it: condA (int8 [3 gates][n][na + 8], float [n][3*na]), condB [n][3*NB],
-// raw LPC [n][16]
-struct CondFrame { float *A, *B, *L; };
+// The per-stream state as one field table: allocation, copies, resets, roll-backs and the by-value record all follow it.
+// `part` says which operations touch a field: reset_signal clears SIGNAL only (the RNG belongs to the sample rate, but
+// lpcnet_reset_signal keeps it, lpcnet.c:226-233); FRAME is the 100 Hz state; TAIL is the stream's row of the conditioning
+// frame a tail reads (the reference's gru_a_condition / gru_b_condition / lpc).
+enum : unsigned { SIGNAL = 1, RNG = 2, FRAME = 4, TAIL = 8, STATE = SIGNAL | RNG | FRAME, ALL = STATE | TAIL };
+// Word i of stream s: base[(i / width) * n * pitch + s * pitch + i % width].  `slot` is the owner's pointer (allocation, freeing).
+struct Field { float *base; int planes, width, pitch; unsigned part; void **slot; };
+// record order: the exported words (oracle_export_state), then the tail part a copy between batches adds
+enum { F_HA, F_HB, F_LAST_SIG, F_DEEMPH, F_CONV1, F_CONV2, F_LPC_CARRY, F_VQ_MEM, F_LAST_EXC, F_FRAME_COUNT, F_RNG, F_COND_A, F_COND_B, F_COND_L, NFIELDS };
+struct Fields { Field f[NFIELDS]; int n; };
 
-// words of one stream's exported state: floats hA[na] hB[16] last_sig[16] deemph conv1[168] conv2[256] lpc_carry[2][16] vq_mem[18],
-// then ints last_exc, frame_count, rng[4]
-__host__ __device__ inline int state_words(int na) { return na + NB + LPC_ORDER + 1 + 2 * FRAME_IN + 2 * COND + 2 * LPC_ORDER + NB_BANDS + 6; }
-// words a copy between batches adds behind them: the stream's row of the frame a tail reads, condA[3*na] condB[3*NB] raw LPC[16]
-__host__ __device__ inline int tail_words(int na) { return 3 * na + 3 * NB + LPC_ORDER; }
+static Fields state_fields(SampleState &ss, FrameState &fs, CondFrame &tail, int n, int na, int a_float)
+{
+    auto field = [](auto *&p, int planes, int width, int pitch, unsigned part) { return Field{(float *)p, planes, width, pitch, part, (void **)&p}; };
+    auto soa = [&](auto *&p, int count, unsigned part) { return field(p, count, 1, 1, part); };        // [count][n]
+    auto row = [&](auto *&p, int count, unsigned part) { return field(p, 1, count, count, part); };    // [n][count]
+    return Fields{{soa(ss.hA, na, SIGNAL), soa(ss.hB, NB, SIGNAL), soa(ss.last_sig, LPC_ORDER, SIGNAL), soa(ss.deemph, 1, SIGNAL),
+                   row(fs.conv1_state, 2 * FRAME_IN, FRAME), row(fs.conv2_state, 2 * COND, FRAME), field(fs.lpc_carry, 2, LPC_ORDER, LPC_ORDER, FRAME),
+                   row(fs.vq_mem, NB_BANDS, FRAME), soa(ss.last_exc, 1, SIGNAL), row(fs.frame_count, 1, FRAME), soa(ss.rng, 4, RNG),
+                   a_float ? row(tail.A, 3 * na, TAIL) : field(tail.A, 3, na, na + 8, TAIL), row(tail.B, 3 * NB, TAIL), row(tail.L, LPC_ORDER, TAIL)}, n};
+}
+// words of the record in front of field `end` (NFIELDS: the whole record)
+static int record_words(const Fields &t, int end)
+{
+    int w = 0;
+    for (int j = 0; j < end; j++) w += t.f[j].planes * t.f[j].width;
+    return w;
+}
+static int record_words(int na, int end) { SampleState ss{}; FrameState fs{}; CondFrame tail{}; return record_words(state_fields(ss, fs, tail, 0, na, 0), end); }
+// words of one stream's exported state, and the words a copy between batches adds behind them
+static int state_words(int na) { return record_words(na, F_COND_A); }
+static int tail_words(int na) { return record_words(na, NFIELDS) - state_words(na); }
 
-// The by-value record of stream s, the one place that knows its layout: the exported words in the order above, then, if `tail`
-// is given, the stream's row of that conditioning frame (a_float: the float flavour's condA layout).  UNPACK: record -> stream.
+static size_t field_floats(const Field &f, size_t n) { return (size_t)f.planes * n * f.pitch; }
+static bool alloc_state(const Fields &t, unsigned parts)
+{
+    for (const Field &f : t.f) if ((f.part & parts) && !*f.slot && cudaMalloc(f.slot, sizeof(float) * field_floats(f, t.n)) != cudaSuccess) return false;
+    return true;
+}
+static void free_state(const Fields &t)
+{
+    for (const Field &f : t.f) if (f.slot && *f.slot) { cudaFree(*f.slot); *f.slot = nullptr; }
+}
+static int copy_state(const Fields &dst, const Fields &src, unsigned parts, cudaStream_t st)
+{
+    for (int j = 0; j < NFIELDS; j++)
+        if (src.f[j].part & parts)
+            CK(cudaMemcpyAsync(dst.f[j].base, src.f[j].base, sizeof(float) * field_floats(src.f[j], src.n), cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+// per-stream state kernels (rare paths: resets, export / import, copies between batches, mixed silent segments, partial flushes)
+__device__ inline size_t field_word(const Field &f, size_t n, size_t s, int i) { return (size_t)(i / f.width) * n * f.pitch + s * f.pitch + i % f.width; }
+// one block per record k of buf (`words` apart; 0: every stream reads the same record): stream rows[k] (rows == NULL: stream s0 + k).
+// The fields of `parts` move, each at its place in the record.  UNPACK: record -> stream.
 template <bool UNPACK>
-__device__ void move_record(const StateView &v, size_t s, float *rec, const CondFrame &tail, int a_float)
-{
-    const size_t n = v.n;
-    int o = 0;
-    auto mv = [&](float *base, size_t stride, int count, size_t off) {
-        for (int i = threadIdx.x; i < count; i += blockDim.x) { float *p = base + off + (size_t)i * stride; if (UNPACK) *p = rec[o + i]; else rec[o + i] = *p; }
-        o += count;
-    };
-    mv(v.ss.hA, n, v.na, s); mv(v.ss.hB, n, NB, s); mv(v.ss.last_sig, n, LPC_ORDER, s); mv(v.ss.deemph, 1, 1, s);
-    mv(v.fs.conv1_state, 1, 2 * FRAME_IN, s * 2 * FRAME_IN); mv(v.fs.conv2_state, 1, 2 * COND, s * 2 * COND);
-    mv(v.fs.lpc_carry, 1, LPC_ORDER, s * LPC_ORDER); mv(v.fs.lpc_carry, 1, LPC_ORDER, (n + s) * LPC_ORDER);
-    mv(v.fs.vq_mem, 1, NB_BANDS, s * NB_BANDS);
-    mv(reinterpret_cast<float *>(v.ss.last_exc), 1, 1, s); mv(reinterpret_cast<float *>(v.fs.frame_count), 1, 1, s);
-    mv(reinterpret_cast<float *>(v.ss.rng), n, 4, s);
-    if (!tail.A) return;
-    const int na = v.na;
-    if (a_float) mv(tail.A, 1, 3 * na, s * 3 * na);
-    else for (int g = 0; g < 3; g++) mv(tail.A, 1, na, (g * n + s) * (na + 8));
-    mv(tail.B, 1, 3 * NB, s * 3 * NB);
-    mv(tail.L, 1, LPC_ORDER, s * LPC_ORDER);
-}
-// one block per record k of buf (`words` apart): stream rows[k] (rows == NULL: stream s0 + k)
-__global__ void streams_pack_kernel(StateView v, const int *rows, int s0, float *buf, int words, CondFrame tail, int a_float)
+__global__ void records_kernel(Fields t, const int *rows, int s0, float *buf, int words, unsigned parts)
 {
     const int k = blockIdx.x;
-    move_record<false>(v, rows ? rows[k] : s0 + k, buf + (size_t)k * words, tail, a_float);
-}
-__global__ void streams_unpack_kernel(StateView v, const int *rows, int s0, float *buf, int words, CondFrame tail, int a_float)
-{
-    const int k = blockIdx.x;
-    move_record<true>(v, rows ? rows[k] : s0 + k, buf + (size_t)k * words, tail, a_float);
-}
-
-// lpcnet_reset (lpcnet.c:174-182) for the listed streams (ids == NULL: all n streams); signal_only = lpcnet_reset_signal (lpcnet.c:226-233).
-// A full reset also zeroes the streams' entries of `tail` (the reference clears gru_a_condition, gru_b_condition and lpc), if given.
-__global__ void reset_streams_kernel(StateView v, const int *ids, int count, uint4 seed, int signal_only, CondFrame tail, int a_float)
-{
-    const int k = blockIdx.x;
-    if (k >= count) return;
-    const size_t n = v.n, s = ids ? ids[k] : k;
-    if (!signal_only && tail.A) {
-        const int na = v.na;
-        if (a_float) for (int i = threadIdx.x; i < 3 * na; i += blockDim.x) tail.A[s * 3 * na + i] = 0.f;
-        else for (int i = threadIdx.x; i < 3 * na; i += blockDim.x) tail.A[((i / na) * n + s) * (na + 8) + i % na] = 0.f;
-        for (int i = threadIdx.x; i < 3 * NB; i += blockDim.x) tail.B[s * 3 * NB + i] = 0.f;
-        for (int i = threadIdx.x; i < LPC_ORDER; i += blockDim.x) tail.L[s * LPC_ORDER + i] = 0.f;
-    }
-    for (int i = threadIdx.x; i < v.na; i += blockDim.x) v.ss.hA[i * n + s] = 0.f;
-    for (int i = threadIdx.x; i < NB; i += blockDim.x) { v.ss.hB[i * n + s] = 0.f; v.ss.last_sig[i * n + s] = 0.f; }
-    if (threadIdx.x == 0) { v.ss.deemph[s] = 0.f; v.ss.last_exc[s] = 128; }      // last_exc = lin2ulaw(0.f) = 128 (lpcnet.c:180)
-    if (signal_only) return;
-    for (int i = threadIdx.x; i < 2 * FRAME_IN; i += blockDim.x) v.fs.conv1_state[s * 2 * FRAME_IN + i] = 0.f;
-    for (int i = threadIdx.x; i < 2 * COND; i += blockDim.x) v.fs.conv2_state[s * 2 * COND + i] = 0.f;
-    for (int i = threadIdx.x; i < LPC_ORDER; i += blockDim.x) { v.fs.lpc_carry[s * LPC_ORDER + i] = 0.f; v.fs.lpc_carry[(n + s) * LPC_ORDER + i] = 0.f; }
-    for (int i = threadIdx.x; i < NB_BANDS; i += blockDim.x) v.fs.vq_mem[s * NB_BANDS + i] = 0.f;
-    if (threadIdx.x == 0) {
-        v.fs.frame_count[s] = 0;
-        v.ss.rng[s] = seed.x; v.ss.rng[n + s] = seed.y; v.ss.rng[2 * n + s] = seed.z; v.ss.rng[3 * n + s] = seed.w;
+    const size_t s = rows ? rows[k] : s0 + k;
+    float *rec = buf + (size_t)k * words;
+    for (int j = 0, o = 0; j < NFIELDS; o += t.f[j].planes * t.f[j].width, j++) {
+        const Field &f = t.f[j];
+        if (!(f.part & parts)) continue;
+        for (int i = threadIdx.x; i < f.planes * f.width; i += blockDim.x) {
+            float *p = f.base + field_word(f, t.n, s, i);
+            if (UNPACK) *p = rec[o + i]; else rec[o + i] = *p;
+        }
     }
 }
-
-// after a one-frame launch over a MIXED segment: streams still in their silent warm-up (f < nsil[s]) get their sample-rate
-// state back from the shadow copy and zeros as output (lpcnet.c:239-243: RNN_CLEAR(output), return — nothing advances)
-__global__ void restore_silent_kernel(SampleState cur, SampleState old, const int *nsil, int f, int n, int na, short *pcm, long long pcm_stride, int spf)
+// dst <- src, the fields of `parts`, for the streams s with mask[s] set; their `spf` samples at pcm + s * pcm_stride become zeros (pcm != NULL)
+__global__ void restore_masked_kernel(Fields dst, Fields src, const int *mask, unsigned parts, short *pcm, long long pcm_stride, int spf)
 {
-    const int s = blockIdx.x;
-    if (s >= n || f >= nsil[s]) return;
-    const size_t nn = n;
-    for (int i = threadIdx.x; i < na; i += blockDim.x) cur.hA[i * nn + s] = old.hA[i * nn + s];
-    for (int i = threadIdx.x; i < NB; i += blockDim.x) { cur.hB[i * nn + s] = old.hB[i * nn + s]; cur.last_sig[i * nn + s] = old.last_sig[i * nn + s]; }
-    if (threadIdx.x < 4) cur.rng[threadIdx.x * nn + s] = old.rng[threadIdx.x * nn + s];
-    if (threadIdx.x == 0) { cur.deemph[s] = old.deemph[s]; cur.last_exc[s] = old.last_exc[s]; }
-    for (int i = threadIdx.x; i < spf; i += blockDim.x) pcm[(size_t)s * pcm_stride + i] = 0;
-}
-
-// after a one-frame launch of a flush: streams that sit the frame out (keep[s]) get their 100 Hz state back from the shadow copy
-__global__ void keep_frame_state_kernel(FrameState cur, FrameState old, const int *keep, int n)
-{
-    const int s = blockIdx.x;
-    if (s >= n || !keep[s]) return;
-    for (int i = threadIdx.x; i < 2 * FRAME_IN; i += blockDim.x) cur.conv1_state[(size_t)s * 2 * FRAME_IN + i] = old.conv1_state[(size_t)s * 2 * FRAME_IN + i];
-    for (int i = threadIdx.x; i < 2 * COND; i += blockDim.x) cur.conv2_state[(size_t)s * 2 * COND + i] = old.conv2_state[(size_t)s * 2 * COND + i];
-    for (int i = threadIdx.x; i < LPC_ORDER; i += blockDim.x) {
-        cur.lpc_carry[(size_t)s * LPC_ORDER + i] = old.lpc_carry[(size_t)s * LPC_ORDER + i];
-        cur.lpc_carry[((size_t)n + s) * LPC_ORDER + i] = old.lpc_carry[((size_t)n + s) * LPC_ORDER + i];
+    const size_t s = blockIdx.x;
+    if (!mask[s]) return;
+    for (int j = 0; j < NFIELDS; j++) {
+        const Field &f = dst.f[j];
+        if (!(f.part & parts)) continue;
+        for (int i = threadIdx.x; i < f.planes * f.width; i += blockDim.x) {
+            const size_t w = field_word(f, dst.n, s, i);
+            f.base[w] = src.f[j].base[w];
+        }
     }
-    if (threadIdx.x == 0) cur.frame_count[s] = old.frame_count[s];
+    if (pcm) for (int i = threadIdx.x; i < spf; i += blockDim.x) pcm[s * pcm_stride + i] = 0;
 }
 
-static StateView view_of(LPCNetB200Batch *b) { return StateView{b->n, b->model.na, b->ss, b->fs}; }
-
-static size_t condA_floats(const LPCNetB200Batch *b) { return condA_frame_floats(b->model.is_float != 0, b->n, b->model.na); }
 // the conditioning the per-sample kernel reads for the frame in slot `pos`; frame f of a chunk reads lpc_raw entry f + 2 - d
 // (frame_kernels.cu), TAIL_SLOT its own entry
 static CondFrame frame_at(const LPCNetB200Batch *b, int pos)
@@ -281,70 +260,23 @@ static CondFrame frame_at(const LPCNetB200Batch *b, int pos)
     const size_t n = b->n;
     const int d = b->model.cfg.end2end ? 0 : b->model.cfg.features_delay;
     const size_t e = pos == TAIL_SLOT ? CHUNK + 2 : pos + 2 - d;
-    return CondFrame{b->condA + pos * condA_floats(b), b->condB + pos * n * 3 * NB, b->lpc_raw + e * n * LPC_ORDER};
+    return CondFrame{b->condA + pos * condA_frame_floats(b->model.is_float != 0, n, b->model.na), b->condB + pos * n * 3 * NB, b->lpc_raw + e * n * LPC_ORDER};
 }
-static int copy_cond_frame(const LPCNetB200Batch *b, const CondFrame &dst, const CondFrame &src, cudaStream_t st)
+// the batch's state, with the frame in slot `pos` as its tail (pos < 0: none).  The tail is not the batch's own allocation: no slots.
+static Fields batch_fields(LPCNetB200Batch *b, int pos)
 {
-    CK(cudaMemcpyAsync(dst.A, src.A, sizeof(float) * condA_floats(b), cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.B, src.B, sizeof(float) * b->n * 3 * NB, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.L, src.L, sizeof(float) * b->n * LPC_ORDER, cudaMemcpyDeviceToDevice, st));
-    return 0;
+    CondFrame tail = pos >= 0 ? frame_at(b, pos) : CondFrame{};
+    Fields t = state_fields(b->ss, b->fs, tail, b->n, b->model.na, b->model.is_float);
+    for (int j = F_COND_A; j < NFIELDS; j++) t.f[j].slot = nullptr;
+    return t;
 }
+static Fields shadow_fields(LPCNetB200Batch *b) { return state_fields(b->shadow.ss, b->shadow.fs, b->shadow.tail, b->n, b->model.na, b->model.is_float); }
 // move the frame a tail reads into TAIL_SLOT, out of the chunk slots the next frame-network run overwrites
 static int park_tail(LPCNetB200Batch *b, cudaStream_t st)
 {
     if (b->cond_last < 0 || b->cond_last == TAIL_SLOT) return 0;
-    if (copy_cond_frame(b, frame_at(b, TAIL_SLOT), frame_at(b, b->cond_last), st)) return -1;
+    if (copy_state(batch_fields(b, TAIL_SLOT), batch_fields(b, b->cond_last), TAIL, st)) return -1;
     b->cond_last = TAIL_SLOT;
-    return 0;
-}
-
-static bool alloc_frame_state(FrameState *fs, size_t n)
-{
-    bool ok = true;
-    auto al = [&](void **p, size_t bytes) { if (ok && cudaMalloc(p, bytes) != cudaSuccess) ok = false; };
-    al((void **)&fs->conv1_state, sizeof(float) * 2 * FRAME_IN * n); al((void **)&fs->conv2_state, sizeof(float) * 2 * COND * n);
-    al((void **)&fs->lpc_carry, sizeof(float) * 2 * LPC_ORDER * n); al((void **)&fs->vq_mem, sizeof(float) * NB_BANDS * n);
-    al((void **)&fs->frame_count, sizeof(int) * n);
-    return ok;
-}
-static void free_frame_state(FrameState *fs)
-{
-    void *p[] = {fs->conv1_state, fs->conv2_state, fs->lpc_carry, fs->vq_mem, fs->frame_count};
-    for (void *q : p) if (q) cudaFree(q);
-    fs->conv1_state = fs->conv2_state = fs->lpc_carry = fs->vq_mem = nullptr; fs->frame_count = nullptr;
-}
-static int copy_frame_state(const FrameState &dst, const FrameState &src, size_t n, cudaStream_t st)
-{
-    CK(cudaMemcpyAsync(dst.conv1_state, src.conv1_state, sizeof(float) * 2 * FRAME_IN * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.conv2_state, src.conv2_state, sizeof(float) * 2 * COND * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.lpc_carry, src.lpc_carry, sizeof(float) * 2 * LPC_ORDER * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.vq_mem, src.vq_mem, sizeof(float) * NB_BANDS * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.frame_count, src.frame_count, sizeof(int) * n, cudaMemcpyDeviceToDevice, st));
-    return 0;
-}
-
-static int alloc_sample_state(SampleState *ss, size_t n, int na)
-{
-    CK(cudaMalloc((void **)&ss->hA, sizeof(float) * na * n)); CK(cudaMalloc((void **)&ss->hB, sizeof(float) * NB * n));
-    CK(cudaMalloc((void **)&ss->last_sig, sizeof(float) * LPC_ORDER * n)); CK(cudaMalloc((void **)&ss->deemph, sizeof(float) * n));
-    CK(cudaMalloc((void **)&ss->last_exc, sizeof(int) * n)); CK(cudaMalloc((void **)&ss->rng, sizeof(uint32_t) * 4 * n));
-    return 0;
-}
-static void free_sample_state(SampleState *ss)
-{
-    void *p[] = {ss->hA, ss->hB, ss->last_sig, ss->deemph, ss->last_exc, ss->rng};
-    for (void *q : p) if (q) cudaFree(q);
-    memset(ss, 0, sizeof(*ss));
-}
-static int copy_sample_state(const SampleState &dst, const SampleState &src, size_t n, int na, cudaStream_t st)
-{
-    CK(cudaMemcpyAsync(dst.hA, src.hA, sizeof(float) * na * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.hB, src.hB, sizeof(float) * NB * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.last_sig, src.last_sig, sizeof(float) * LPC_ORDER * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.deemph, src.deemph, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.last_exc, src.last_exc, sizeof(int) * n, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(dst.rng, src.rng, sizeof(uint32_t) * 4 * n, cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 
@@ -360,30 +292,35 @@ int lpcnet_b200_device_count(void)
     return c;
 }
 
+// lpcnet_reset (lpcnet.c:174-182) for the listed streams (ids == NULL: all n streams); signal_only = lpcnet_reset_signal (lpcnet.c:226-233).
+// A fresh record is unpacked into every listed stream: zeros, last_exc = lin2ulaw(0.f) = 128 (lpcnet.c:180), the kiss99 seed of the RNG.
 static int reset_impl(LPCNetB200Batch *b, const int *ids, int count, int signal_only)
 {
     CK(cudaSetDevice(b->device));
-    if (order_enter(b, b->stream)) return -1;
+    if (ids) for (int k = 0; k < count; k++) if (ids[k] < 0 || ids[k] >= b->n) { set_error("reset_streams: stream %d out of range", ids[k]); return -1; }
+    // a full reset of every stream leaves the zeroed TAIL_SLOT as what a tail reads; a per-stream one zeroes the streams' part of
+    // the current tail frame (as the reference clears gru_a_condition, gru_b_condition and lpc; none since an import: tails stay
+    // refused until the next frame-network run)
+    if (!signal_only && !ids) b->cond_last = TAIL_SLOT;
+    const Fields t = batch_fields(b, b->cond_last);
+    const int words = record_words(t, NFIELDS), last_exc = 128;
     uint32_t seed[4];
     kiss99_seed(seed);
-    int *d_ids = nullptr;
-    if (ids) {
-        for (int k = 0; k < count; k++) if (ids[k] < 0 || ids[k] >= b->n) { set_error("reset_streams: stream %d out of range", ids[k]); return -1; }
-        CK(cudaMalloc((void **)&d_ids, sizeof(int) * count));
-        CK(cudaMemcpyAsync(d_ids, ids, sizeof(int) * count, cudaMemcpyHostToDevice, b->stream));
-    }
-    // a full reset of every stream leaves the zeroed TAIL_SLOT as what a tail reads; a per-stream one zeroes the streams' part of
-    // the current tail frame (none since an import: tails stay refused until the next frame-network run)
-    if (!signal_only && !ids) b->cond_last = TAIL_SLOT;
-    const CondFrame tail = b->cond_last >= 0 ? frame_at(b, b->cond_last) : CondFrame{nullptr, nullptr, nullptr};
-    reset_streams_kernel<<<count, 128, 0, b->stream>>>(view_of(b), d_ids, count, make_uint4(seed[0], seed[1], seed[2], seed[3]), signal_only,
-                                                       tail, b->model.is_float);
+    std::vector<float> rec(words, 0.f);
+    memcpy(&rec[record_words(t, F_LAST_EXC)], &last_exc, sizeof(last_exc));
+    memcpy(&rec[record_words(t, F_RNG)], seed, sizeof(seed));
+    // staging: the record, then the stream ids
+    if (ensure(b, (void **)&b->d_state, &b->d_state_cap, sizeof(float) * words + (ids ? sizeof(int) * count : 0))) return -1;
+    int *d_ids = ids ? reinterpret_cast<int *>(b->d_state + words) : nullptr;
+    if (order_enter(b, b->stream)) return -1;
+    CK(cudaMemcpyAsync(b->d_state, rec.data(), sizeof(float) * words, cudaMemcpyHostToDevice, b->stream));
+    if (ids) CK(cudaMemcpyAsync(d_ids, ids, sizeof(int) * count, cudaMemcpyHostToDevice, b->stream));
+    records_kernel<true><<<count, 128, 0, b->stream>>>(t, d_ids, 0, b->d_state, 0, signal_only ? SIGNAL : b->cond_last >= 0 ? ALL : STATE);
     if (order_leave(b, b->stream)) return -1;
     CK(cudaStreamSynchronize(b->stream));
-    if (d_ids) cudaFree(d_ids);
     if (!signal_only) {
-        if (ids) for (int k = 0; k < count; k++) { (*b->fc)[ids[k]] = 0; (*b->dfill)[ids[k]] = 0; }
-        else { std::fill(b->fc->begin(), b->fc->end(), 0); std::fill(b->dfill->begin(), b->dfill->end(), 0); b->deferred_fill = 0; }
+        if (ids) for (int k = 0; k < count; k++) { b->fc[ids[k]] = 0; b->dfill[ids[k]] = 0; }
+        else { std::fill(b->fc.begin(), b->fc.end(), 0); std::fill(b->dfill.begin(), b->dfill.end(), 0); b->deferred_fill = 0; }
     }
     return 0;
 }
@@ -411,18 +348,21 @@ LPCNetB200Batch *lpcnet_b200_batch_create_ex(int n_streams, const unsigned char 
     if (cnt <= 0) { set_error("no CUDA device available (this engine has no CPU fallback)"); return nullptr; }
     if (device < 0 || device >= cnt) { set_error("device %d out of range (%d devices)", device, cnt); return nullptr; }
     if (cudaSetDevice(device) != cudaSuccess) { set_error("cudaSetDevice(%d) failed", device); return nullptr; }
-    LPCNetB200Batch *b = (LPCNetB200Batch *)calloc(1, sizeof(*b));
+    LPCNetB200Batch *b = new LPCNetB200Batch();
     b->device = device; b->n = n_streams; b->cond_last = -1;
-    b->kev = new std::vector<cudaEvent_t>();
-    b->fc = new std::vector<int>(n_streams, 0);
-    b->deferred = new std::vector<float>();
-    b->dfill = new std::vector<int>(n_streams, 0);
+    b->fc.assign(n_streams, 0);
+    b->dfill.assign(n_streams, 0);
     ModelConfig mc{-1.f, -1, -1};
     if (cfg) { mc.lpc_gamma = cfg->lpc_gamma; mc.features_delay = cfg->features_delay; mc.end2end = cfg->end2end; }
-    if (model_load(&b->model, blob, blob_len, &mc) != 0) { delete b->kev; delete b->fc; delete b->deferred; delete b->dfill; free(b); return nullptr; }
+    if (model_load(&b->model, blob, blob_len, &mc) != 0) { delete b; return nullptr; }
     const size_t n = n_streams;
     const int na = b->model.na;
-    bool ok = alloc_sample_state(&b->ss, n, na) == 0 && alloc_frame_state(&b->fs, n);
+    // the exported record is oracle_export_state's (lpcnet_b200_batch_state_size); a copy between batches adds the tail part
+    if (state_words(na) != na + 513 || tail_words(na) != 3 * na + 64) {
+        set_error("state record of %d words + %d tail words, expected %d + %d", state_words(na), tail_words(na), na + 513, 3 * na + 64);
+        lpcnet_b200_batch_destroy(b); return nullptr;
+    }
+    bool ok = alloc_state(batch_fields(b, -1), STATE);
     auto al = [&](void **p, size_t bytes) { if (ok && cudaMalloc(p, bytes) != cudaSuccess) ok = false; };
     al((void **)&b->fs.work, sizeof(float) * frame_work_floats(n));
     al((void **)&b->condA, sizeof(float) * (size_t)(CHUNK + 1) * condA_frame_floats(b->model.is_float != 0, n, na)); al((void **)&b->condB, sizeof(float) * (size_t)(CHUNK + 1) * n * 3 * NB);
@@ -468,18 +408,16 @@ void lpcnet_b200_batch_destroy(LPCNetB200Batch *b)
     if (b->sink_stream) { cudaStreamSynchronize(b->sink_stream); cudaStreamDestroy(b->sink_stream); }
     if (b->sink_ev) cudaEventDestroy(b->sink_ev);
     if (b->sink_done) cudaEventDestroy(b->sink_done);
-    free_sample_state(&b->ss); free_sample_state(&b->shadow);
-    free_frame_state(&b->fs); free_frame_state(&b->fshadow);
-    void *ptrs[] = {b->fs.work, b->condA, b->condB, b->lpc_raw, b->d_features, b->d_pcm, b->d_packets, b->d_state, b->d_nsil, b->d_keep};
+    free_state(batch_fields(b, -1)); free_state(shadow_fields(b));
+    void *ptrs[] = {b->fs.work, b->condA, b->condB, b->lpc_raw, b->d_features, b->d_pcm, b->d_packets, b->d_state, b->d_mask};
     for (void *p : ptrs) if (p) cudaFree(p);
-    if (b->kev) { for (cudaEvent_t e : *b->kev) cudaEventDestroy(e); delete b->kev; }
-    delete b->fc; delete b->deferred; delete b->dfill;
+    for (cudaEvent_t e : b->kev) cudaEventDestroy(e);
     model_free(&b->model);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
     if (b->order_ev) cudaEventDestroy(b->order_ev);
     if (b->stream) cudaStreamDestroy(b->stream);
-    free(b);
+    delete b;
 }
 
 int lpcnet_b200_batch_streams(const LPCNetB200Batch *b) { return b ? b->n : 0; }
@@ -527,20 +465,20 @@ static SampleParams sample_params(const LPCNetB200Batch *b, int pos, int nf, int
 static bool batch_fast_cvt(const LPCNetB200Batch *b) { return b->model.fast_cvt && !b->env_exact_cvt; }
 
 // an event pair around a per-sample launch, resolved lazily by lpcnet_b200_*_last_sample_kernel_ms (no sync here)
-static int time_launch(std::vector<cudaEvent_t> *kev, int *used, cudaStream_t st)
+static int time_launch(std::vector<cudaEvent_t> &kev, int *used, cudaStream_t st)
 {
-    while ((int)kev->size() < *used + 1) { cudaEvent_t e; CK(cudaEventCreate(&e)); kev->push_back(e); }
-    CK(cudaEventRecord((*kev)[*used], st));
+    while ((int)kev.size() < *used + 1) { cudaEvent_t e; CK(cudaEventCreate(&e)); kev.push_back(e); }
+    CK(cudaEventRecord(kev[*used], st));
     ++*used;
     return 0;
 }
-static float timed_ms(const std::vector<cudaEvent_t> *kev, int used)
+static float timed_ms(const std::vector<cudaEvent_t> &kev, int used)
 {
     float total = 0.f;
     for (int i = 0; i + 1 < used; i += 2) {
         float ms = 0.f;
-        if (cudaEventSynchronize((*kev)[i + 1]) != cudaSuccess) return -1.f;
-        if (cudaEventElapsedTime(&ms, (*kev)[i], (*kev)[i + 1]) != cudaSuccess) return -1.f;
+        if (cudaEventSynchronize(kev[i + 1]) != cudaSuccess) return -1.f;
+        if (cudaEventElapsedTime(&ms, kev[i], kev[i + 1]) != cudaSuccess) return -1.f;
         total += ms;
     }
     return total;
@@ -582,24 +520,27 @@ static int sample_prefix(LPCNetB200Batch *b, int pos0, int nf, int spf, short *p
 {
     const int n = b->n, delay = b->model.cfg.features_delay;
     int fc_min = 1 << 30, fc_max = 0;
-    for (int v : *b->fc) { fc_min = std::min(fc_min, v); fc_max = std::max(fc_max, v); }
+    for (int v : b->fc) { fc_min = std::min(fc_min, v); fc_max = std::max(fc_max, v); }
     const int sil_all = std::min(nf, std::max(0, delay - fc_max));     // frames silent for EVERY stream
     const int sil_any = std::min(nf, std::max(0, delay - fc_min));     // frames silent for at least one stream
     int launches = 0;
     if (sil_all > 0) CK(cudaMemset2DAsync(pcm, pcm_stride * sizeof(short), 0, (size_t)sil_all * spf * sizeof(short), n, st));
     if (sil_any > sil_all) {
         // mixed segment (some streams were reset later than others): one launch per frame over all streams, then the streams
-        // that are still silent get their state back and zeros as output
-        if (!b->shadow.hA && alloc_sample_state(&b->shadow, n, b->model.na)) return -1;
-        if (!b->d_nsil) CK(cudaMalloc((void **)&b->d_nsil, sizeof(int) * n));
-        std::vector<int> nsil(n);
-        for (int s = 0; s < n; s++) nsil[s] = std::min(nf, std::max(0, delay - (*b->fc)[s]));
-        CK(cudaMemcpyAsync(b->d_nsil, nsil.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
-        CK(cudaStreamSynchronize(st));                              // (nsil is a stack vector; this path runs at most FEATURES_DELAY times per reset)
+        // that are still silent get their sample-rate state back and zeros as output (lpcnet.c:239-243: RNN_CLEAR(output),
+        // return — nothing advances)
+        static_assert(MAX_FEATURES_DELAY <= DEFER_MAX, "silent frames of a segment fit the mask");
+        if (!alloc_state(shadow_fields(b), SIGNAL | RNG)) { set_error("mixed silent segment: device allocation failed"); return -1; }
+        const Fields cur = batch_fields(b, -1), old = shadow_fields(b);
+        if (!b->d_mask) CK(cudaMalloc((void **)&b->d_mask, sizeof(int) * DEFER_MAX * n));
+        std::vector<int> silent((size_t)sil_any * n);                 // [f][s]: stream s is still silent in frame f
+        for (int f = 0; f < sil_any; f++) for (int s = 0; s < n; s++) silent[(size_t)f * n + s] = f < delay - b->fc[s];
+        CK(cudaMemcpyAsync(b->d_mask, silent.data(), sizeof(int) * silent.size(), cudaMemcpyHostToDevice, st));
+        CK(cudaStreamSynchronize(st));                              // (silent is a stack vector; this path runs at most FEATURES_DELAY times per reset)
         for (int f = sil_all; f < sil_any; f++) {
-            if (copy_sample_state(b->shadow, b->ss, n, b->model.na, st)) return -1;
+            if (copy_state(old, cur, SIGNAL | RNG, st)) return -1;
             if (launch_sample(b, pos0 + f, 1, spf, pcm + (size_t)f * spf, pcm_stride, f == 0 ? preload : 0, st, true)) return -1;
-            restore_silent_kernel<<<n, 128, 0, st>>>(b->ss, b->shadow, b->d_nsil, f, n, b->model.na, pcm + (size_t)f * spf, pcm_stride, spf);
+            restore_masked_kernel<<<n, 128, 0, st>>>(cur, old, b->d_mask + (size_t)f * n, SIGNAL | RNG, pcm + (size_t)f * spf, pcm_stride, spf);
             launches += 2;
         }
     }
@@ -615,7 +556,7 @@ static int sample_frames(LPCNetB200Batch *b, int pos0, int nf, int spf, short *p
         if (launch_sample(b, pos0 + sil_any, nf - sil_any, spf, pcm + (size_t)sil_any * spf, pcm_stride, sil_any == 0 ? preload : 0, st, true)) return -1;
         launches += 1;
     }
-    for (int &v : *b->fc) v = std::min(1000, v + nf);
+    for (int &v : b->fc) v = std::min(1000, v + nf);
     return launches;
 }
 
@@ -737,7 +678,7 @@ int lpcnet_b200_batch_run_frame_network(LPCNetB200Batch *b, const float *feature
         launch_frame_network(b->model, b->fs, b->d_features + (size_t)c0 * feature_stride, (long long)nframes * feature_stride, feature_stride, b->n, nf,
                              b->condA, b->condB, b->lpc_raw, b->stream);
         b->cond_last = nf - 1;
-        for (int &v : *b->fc) v = std::min(1000, v + nf);
+        for (int &v : b->fc) v = std::min(1000, v + nf);
     }
     if (order_leave(b, b->stream)) return -1;
     CK(cudaStreamSynchronize(b->stream));
@@ -763,10 +704,10 @@ int lpcnet_b200_batch_synthesize_tail(LPCNetB200Batch *b, int samples, short *pc
     b->kev_used = 0;
     // the frame counters were already advanced by the frame network run; the silent test of lpcnet.c:239 looks at the CURRENT
     // count, sample_frames() at the count before the frame: step back by one for the duration of the call
-    std::vector<int> saved = *b->fc;
-    for (int &v : *b->fc) v = v - 1;
+    std::vector<int> saved = b->fc;
+    for (int &v : b->fc) v = v - 1;
     const int r = sample_frames(b, b->cond_last, 1, samples, b->d_pcm, samples, preload, b->stream);
-    *b->fc = saved;
+    b->fc = saved;
     if (r < 0) return -1;
     b->last_launches = r;
     if (order_leave(b, b->stream)) return -1;
@@ -782,11 +723,11 @@ int lpcnet_b200_batch_frame_network_deferred(LPCNetB200Batch *b, const float *fe
 {
     if (!b || !features || feature_stride < NB_FEAT) { set_error("frame_network_deferred: bad arguments"); return -1; }
     const size_t fr = (size_t)b->n * NB_FEAT;
-    b->deferred->resize(fr * DEFER_MAX);
-    float *q = b->deferred->data();
+    b->deferred.resize(fr * DEFER_MAX);
+    float *q = b->deferred.data();
     if (b->deferred_fill == DEFER_MAX) memmove(q, q + fr, sizeof(float) * fr * (DEFER_MAX - 1));
     else b->deferred_fill++;
-    for (int &v : *b->dfill) v = std::min(DEFER_MAX, v + 1);
+    for (int &v : b->dfill) v = std::min(DEFER_MAX, v + 1);
     float *dst = q + fr * (b->deferred_fill - 1);
     for (int s = 0; s < b->n; s++) memcpy(dst + (size_t)s * NB_FEAT, features + (size_t)s * feature_stride, sizeof(float) * NB_FEAT);
     return 0;
@@ -795,9 +736,9 @@ int lpcnet_b200_batch_frame_network_flush(LPCNetB200Batch *b)
 {
     if (!b) { set_error("null batch"); return -1; }
     const int F = b->deferred_fill, n = b->n;
-    const std::vector<int> fill = *b->dfill;
+    const std::vector<int> fill = b->dfill;
     b->deferred_fill = 0;
-    std::fill(b->dfill->begin(), b->dfill->end(), 0);
+    std::fill(b->dfill.begin(), b->dfill.end(), 0);
     // stream s runs queued frame k iff k >= F - fill[s]; from frame k_all on every stream does
     int k0 = F, k_all = 0;
     for (int v : fill) { k0 = std::min(k0, F - v); k_all = std::max(k_all, F - v); }
@@ -807,28 +748,31 @@ int lpcnet_b200_batch_frame_network_flush(LPCNetB200Batch *b)
     std::vector<float> f((size_t)n * F * NB_FEAT);                   // [n][F][20]
     std::vector<int> keep((size_t)F * n);                            // [F][n]
     for (int k = 0; k < F; k++) for (int s = 0; s < n; s++) {
-        memcpy(&f[((size_t)s * F + k) * NB_FEAT], b->deferred->data() + fr * k + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
+        memcpy(&f[((size_t)s * F + k) * NB_FEAT], b->deferred.data() + fr * k + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
         keep[(size_t)k * n + s] = k < F - fill[s];
     }
     if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * f.size())) return -1;
     if (k_all > k0) {
-        if (!b->fshadow.conv1_state && !alloc_frame_state(&b->fshadow, n)) { set_error("flush: device allocation failed"); return -1; }
-        if (!b->d_keep) CK(cudaMalloc((void **)&b->d_keep, sizeof(int) * DEFER_MAX * n));
+        if (!alloc_state(shadow_fields(b), FRAME)) { set_error("flush: device allocation failed"); return -1; }
+        if (!b->d_mask) CK(cudaMalloc((void **)&b->d_mask, sizeof(int) * DEFER_MAX * n));
     }
     cudaStream_t st = b->stream;
     if (order_enter(b, st)) return -1;
     CK(cudaMemcpyAsync(b->d_features, f.data(), sizeof(float) * f.size(), cudaMemcpyHostToDevice, st));
-    if (k_all > k0) CK(cudaMemcpyAsync(b->d_keep, keep.data(), sizeof(int) * keep.size(), cudaMemcpyHostToDevice, st));
+    if (k_all > k0) CK(cudaMemcpyAsync(b->d_mask, keep.data(), sizeof(int) * keep.size(), cudaMemcpyHostToDevice, st));
     if (park_tail(b, st)) return -1;
-    for (int k = k0; k < k_all; k++) {       // frames only some streams run: one launch per frame, the others' 100 Hz state put back after it
-        if (copy_frame_state(b->fshadow, b->fs, n, st)) return -1;
+    // frames only some streams run: one launch per frame, the others' 100 Hz state put back after it (vq_mem too, which the
+    // frame network does not write: putting it back changes nothing)
+    const Fields cur = batch_fields(b, -1), old = shadow_fields(b);
+    for (int k = k0; k < k_all; k++) {
+        if (copy_state(old, cur, FRAME, st)) return -1;
         launch_frame_network(b->model, b->fs, b->d_features + (size_t)k * NB_FEAT, (long long)F * NB_FEAT, NB_FEAT, n, 1, b->condA, b->condB, b->lpc_raw, st);
-        keep_frame_state_kernel<<<n, 128, 0, st>>>(b->fs, b->fshadow, b->d_keep + (size_t)k * n, n);
+        restore_masked_kernel<<<n, 128, 0, st>>>(cur, old, b->d_mask + (size_t)k * n, FRAME, nullptr, 0, 0);
     }
     if (k_all < F)
         launch_frame_network(b->model, b->fs, b->d_features + (size_t)k_all * NB_FEAT, (long long)F * NB_FEAT, NB_FEAT, n, F - k_all, b->condA, b->condB, b->lpc_raw, st);
     CK(cudaGetLastError());
-    for (int s = 0; s < n; s++) (*b->fc)[s] = std::min(1000, (*b->fc)[s] + fill[s]);
+    for (int s = 0; s < n; s++) b->fc[s] = std::min(1000, b->fc[s] + fill[s]);
     if (order_leave(b, st)) return -1;
     CK(cudaStreamSynchronize(st));                                   // (f and keep are read by the copies above)
     return 0;
@@ -894,7 +838,7 @@ struct LPCNetB200Group {
     bool fast_cvt;                    // conversion-free rounding: only if every member allows it
     uint32_t smem_bytes;              // largest shared-memory footprint of the members
     cudaStream_t stream;
-    std::vector<cudaEvent_t> *kev;    // event pairs around the group's own per-sample launches of the last call
+    std::vector<cudaEvent_t> kev;     // event pairs around the group's own per-sample launches of the last call
     int kev_used, last_launches;
 };
 
@@ -923,7 +867,7 @@ void lpcnet_b200_group_destroy(LPCNetB200Group *g)
     if (!g) return;
     cudaSetDevice(g->device);
     if (g->stream) { cudaStreamSynchronize(g->stream); cudaStreamDestroy(g->stream); }
-    if (g->kev) { for (cudaEvent_t e : *g->kev) cudaEventDestroy(e); delete g->kev; }
+    for (cudaEvent_t e : g->kev) cudaEventDestroy(e);
     delete g;
 }
 
@@ -953,7 +897,6 @@ LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int c
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     const char *e = getenv("LPCNET_B200_STREAMS_PER_CTA");
     g->spc = group_plan(n, count, sms, e ? atoi(e) : 0, &g->ctas);
-    g->kev = new std::vector<cudaEvent_t>();
     if (cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) != cudaSuccess) {
         set_error("group_create: cudaStreamCreate failed"); lpcnet_b200_group_destroy(g); return nullptr;
     }
@@ -1020,7 +963,7 @@ static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_s
         const int r = launch_group(g, live0, nf, spf, pc, pcm_stride, st);
         if (r < 0) return -1;
         launches += r;
-        for (int k = 0; k < g->count; k++) for (int &v : *g->m[k]->fc) v = std::min(1000, v + nf);
+        for (int k = 0; k < g->count; k++) for (int &v : g->m[k]->fc) v = std::min(1000, v + nf);
     }
     CK(cudaGetLastError());
     for (int k = 0; k < g->count; k++) if (order_leave(g->m[k], st)) return -1;
@@ -1274,51 +1217,43 @@ int lpcnet_b200_batch_algorithmic_bytes(const LPCNetB200Batch *b, long *total, l
     return 0;
 }
 
-int lpcnet_b200_batch_get_state(LPCNetB200Batch *b, int s, float *gru_a, float *gru_b, float *last_sig, int *misc, uint32_t *rng)
-{
-    if (!b || s < 0 || s >= b->n) { set_error("bad stream index"); return -1; }
-    CK(cudaSetDevice(b->device));
-    if (order_sync(b)) return -1;
-    const size_t n = b->n;
-    if (gru_a) CK(cudaMemcpy2D(gru_a, sizeof(float), b->ss.hA + s, n * sizeof(float), sizeof(float), b->model.na, cudaMemcpyDeviceToHost));
-    if (gru_b) CK(cudaMemcpy2D(gru_b, sizeof(float), b->ss.hB + s, n * sizeof(float), sizeof(float), NB, cudaMemcpyDeviceToHost));
-    if (last_sig) CK(cudaMemcpy2D(last_sig, sizeof(float), b->ss.last_sig + s, n * sizeof(float), sizeof(float), LPC_ORDER, cudaMemcpyDeviceToHost));
-    if (misc) { CK(cudaMemcpy(&misc[0], b->ss.last_exc + s, sizeof(int), cudaMemcpyDeviceToHost)); misc[1] = (*b->fc)[s]; }
-    if (rng) CK(cudaMemcpy2D(rng, sizeof(uint32_t), b->ss.rng + s, n * sizeof(uint32_t), sizeof(uint32_t), 4, cudaMemcpyDeviceToHost));
-    return 0;
-}
-
 // ---- state by value (what the PLC does with `LPCNetState copy = *st`, lpcnet_plc.c:216-230): one stream <-> host blob ----
 int lpcnet_b200_batch_state_size(const LPCNetB200Batch *b)
 {
     return b ? state_words(b->model.na) * 4 : -1;
 }
-static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
+// stream s's record without the tail part <-> host buffer `rec`, through the staging buffer.  unpack: rec -> stream.
+static int stream_record(LPCNetB200Batch *b, int s, void *rec, bool unpack)
 {
-    if (!b || !buf || s < 0 || s >= b->n) { set_error("state export/import: bad arguments"); return -1; }
-    if (!dir && (*b->dfill)[s] > 0) {
-        set_error("export_state: stream %d has %d queued frames and the exported state has no room for them; flush first", s, (*b->dfill)[s]);
-        return -1;
-    }
     CK(cudaSetDevice(b->device));
-    const size_t bytes = (size_t)state_words(b->model.na) * 4;
+    const Fields t = batch_fields(b, -1);
+    const int words = record_words(t, F_COND_A);
+    const size_t bytes = sizeof(float) * words;
     if (ensure(b, (void **)&b->d_state, &b->d_state_cap, bytes)) return -1;
     if (order_enter(b, b->stream)) return -1;
-    const int words = state_words(b->model.na);
-    const CondFrame none{nullptr, nullptr, nullptr};
-    if (dir) {
-        CK(cudaMemcpyAsync(b->d_state, buf, bytes, cudaMemcpyHostToDevice, b->stream));
-        streams_unpack_kernel<<<1, 128, 0, b->stream>>>(view_of(b), nullptr, s, b->d_state, words, none, 0);
+    if (unpack) {
+        CK(cudaMemcpyAsync(b->d_state, rec, bytes, cudaMemcpyHostToDevice, b->stream));
+        records_kernel<true><<<1, 128, 0, b->stream>>>(t, nullptr, s, b->d_state, words, STATE);
     } else {
-        streams_pack_kernel<<<1, 128, 0, b->stream>>>(view_of(b), nullptr, s, b->d_state, words, none, 0);
-        CK(cudaMemcpyAsync(buf, b->d_state, bytes, cudaMemcpyDeviceToHost, b->stream));
+        records_kernel<false><<<1, 128, 0, b->stream>>>(t, nullptr, s, b->d_state, words, STATE);
+        CK(cudaMemcpyAsync(rec, b->d_state, bytes, cudaMemcpyDeviceToHost, b->stream));
     }
     if (order_leave(b, b->stream)) return -1;
     CK(cudaStreamSynchronize(b->stream));
+    return 0;
+}
+static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
+{
+    if (!b || !buf || s < 0 || s >= b->n) { set_error("state export/import: bad arguments"); return -1; }
+    if (!dir && b->dfill[s] > 0) {
+        set_error("export_state: stream %d has %d queued frames and the exported state has no room for them; flush first", s, b->dfill[s]);
+        return -1;
+    }
+    if (stream_record(b, s, buf, dir)) return -1;
     if (dir) {
-        int fcv; memcpy(&fcv, (const char *)buf + (size_t)(state_words(b->model.na) - 5) * 4, 4);
-        (*b->fc)[s] = fcv;
-        (*b->dfill)[s] = 0;
+        int fcv; memcpy(&fcv, (const char *)buf + sizeof(float) * record_words(batch_fields(b, -1), F_FRAME_COUNT), sizeof(fcv));
+        b->fc[s] = fcv;
+        b->dfill[s] = 0;
         b->cond_last = -1;          // the blob carries no conditioning: no tail until the next frame-network run
     }
     return 0;
@@ -1326,8 +1261,21 @@ static int state_move(LPCNetB200Batch *b, int s, void *buf, int dir)
 int lpcnet_b200_batch_export_state(LPCNetB200Batch *b, int s, void *buf) { return state_move(b, s, buf, 0); }
 int lpcnet_b200_batch_import_state(LPCNetB200Batch *b, int s, const void *buf) { return state_move(b, s, const_cast<void *>(buf), 1); }
 
+// fields of stream s's record; misc = {last_exc, frame counter (from the host mirror)}
+int lpcnet_b200_batch_get_state(LPCNetB200Batch *b, int s, float *gru_a, float *gru_b, float *last_sig, int *misc, uint32_t *rng)
+{
+    if (!b || s < 0 || s >= b->n) { set_error("bad stream index"); return -1; }
+    const Fields t = batch_fields(b, -1);
+    std::vector<float> rec(record_words(t, F_COND_A));
+    if (stream_record(b, s, rec.data(), false)) return -1;
+    auto pick = [&](void *dst, int j) { if (dst) memcpy(dst, &rec[record_words(t, j)], sizeof(float) * t.f[j].planes * t.f[j].width); };
+    pick(gru_a, F_HA); pick(gru_b, F_HB); pick(last_sig, F_LAST_SIG); pick(misc, F_LAST_EXC); pick(rng, F_RNG);
+    if (misc) misc[1] = b->fc[s];
+    return 0;
+}
+
 // ---- whole streams between batches on the device (compaction, shard rebalancing, cloning) ----
-// Each batch's staging buffer d_state holds [count] source rows, [count] destination rows, then the count records (move_record).
+// Each batch's staging buffer d_state holds [count] source rows, [count] destination rows, then the count records (in the order of state_fields).
 // The records are packed on src's stream, copied into dst's staging (peer DMA across devices) and unpacked on dst's stream;
 // staging makes src == dst read every record before any is written.
 static int copy_check(const LPCNetB200Batch *dst, const int *dst_rows, const LPCNetB200Batch *src, const int *src_rows, int count)
@@ -1355,10 +1303,11 @@ int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LP
 {
     if (copy_check(dst, dst_rows, src, src_rows, count)) return -1;
     if (count == 0) return 0;
-    const int na = src->model.na, words = state_words(na) + tail_words(na), a_float = src->model.is_float;
-    const size_t rows_bytes = sizeof(int) * 2 * (size_t)count, bytes = rows_bytes + sizeof(float) * (size_t)count * words;
     const bool tails = dst->cond_last >= 0 && src->cond_last >= 0;      // else dst refuses tails until its next frame-network run
-    const CondFrame none{nullptr, nullptr, nullptr};
+    const Fields ts = batch_fields(src, tails ? src->cond_last : -1), td = batch_fields(dst, tails ? dst->cond_last : -1);
+    const unsigned parts = tails ? ALL : STATE;
+    const int words = record_words(ts, NFIELDS);
+    const size_t rows_bytes = sizeof(int) * 2 * (size_t)count, bytes = rows_bytes + sizeof(float) * (size_t)count * words;
     std::vector<int> rows(2 * (size_t)count);
     std::copy(src_rows, src_rows + count, rows.begin());
     std::copy(dst_rows, dst_rows + count, rows.begin() + count);
@@ -1373,7 +1322,7 @@ int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LP
     float *s_rec = reinterpret_cast<float *>(reinterpret_cast<char *>(src->d_state) + rows_bytes);
     if (order_enter(src, src->stream)) return -1;
     CK(cudaMemcpyAsync(s_rows, rows.data(), rows_bytes, cudaMemcpyHostToDevice, src->stream));
-    streams_pack_kernel<<<count, 128, 0, src->stream>>>(view_of(src), s_rows, 0, s_rec, words, tails ? frame_at(src, src->cond_last) : none, a_float);
+    records_kernel<false><<<count, 128, 0, src->stream>>>(ts, s_rows, 0, s_rec, words, parts);
     CK(cudaGetLastError());
     // 2. src's order event marks the records ready; dst's stream waits for it (and for dst's own last call)
     if (order_leave(src, src->stream)) return -1;
@@ -1389,7 +1338,7 @@ int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LP
         else CK(cudaMemcpyAsync(d_rec, s_rec, bytes - rows_bytes, cudaMemcpyDeviceToDevice, dst->stream));
     }
     // 4. unpack on dst's stream
-    streams_unpack_kernel<<<count, 128, 0, dst->stream>>>(view_of(dst), d_rows + count, 0, d_rec, words, tails ? frame_at(dst, dst->cond_last) : none, a_float);
+    records_kernel<true><<<count, 128, 0, dst->stream>>>(td, d_rows + count, 0, d_rec, words, parts);
     CK(cudaGetLastError());
     // 5. both orders end here; the call returns with the copy complete
     if (order_leave(dst, dst->stream)) return -1;
@@ -1398,16 +1347,16 @@ int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LP
     CK(cudaStreamSynchronize(src->stream));
 
     // host mirrors: frame counters and deferred queues, read from src as it was before the call
-    const std::vector<int> sfc = *src->fc, sfill = *src->dfill;
-    const std::vector<float> sq = *src->deferred;
+    const std::vector<int> sfc = src->fc, sfill = src->dfill;
+    const std::vector<float> sq = src->deferred;
     const int sF = src->deferred_fill;
     int q_max = 0;
     for (int k = 0; k < count; k++) q_max = std::max(q_max, sfill[src_rows[k]]);
     const size_t sfr = (size_t)src->n * NB_FEAT, dfr = (size_t)dst->n * NB_FEAT;
     if (q_max > dst->deferred_fill) {       // grow dst's queue at its old end: the other streams read only their last dfill frames
         const int grow = q_max - dst->deferred_fill;
-        dst->deferred->resize(dfr * DEFER_MAX);
-        float *q = dst->deferred->data();
+        dst->deferred.resize(dfr * DEFER_MAX);
+        float *q = dst->deferred.data();
         memmove(q + dfr * grow, q, sizeof(float) * dfr * dst->deferred_fill);
         std::fill(q, q + dfr * grow, 0.f);
         dst->deferred_fill = q_max;
@@ -1416,9 +1365,9 @@ int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LP
     for (int k = 0; k < count; k++) {
         const int s = src_rows[k], d = dst_rows[k], qn = sfill[s];
         for (int i = 0; i < qn; i++)
-            memcpy(dst->deferred->data() + dfr * (dF - qn + i) + (size_t)d * NB_FEAT, sq.data() + sfr * (sF - qn + i) + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
-        (*dst->dfill)[d] = qn;
-        (*dst->fc)[d] = sfc[s];
+            memcpy(dst->deferred.data() + dfr * (dF - qn + i) + (size_t)d * NB_FEAT, sq.data() + sfr * (sF - qn + i) + (size_t)s * NB_FEAT, sizeof(float) * NB_FEAT);
+        dst->dfill[d] = qn;
+        dst->fc[d] = sfc[s];
     }
     if (!tails) dst->cond_last = -1;
     return 0;
@@ -1427,38 +1376,31 @@ int lpcnet_b200_batch_copy_streams(LPCNetB200Batch *dst, const int *dst_rows, LP
 // ---- whole-batch snapshot on the device (roll-back after speculative synthesis) ----
 // It also holds the frame a tail reads, as the reference's state copy holds gru_a_condition / gru_b_condition / lpc.
 struct LPCNetB200Snapshot {
-    int n, na, device; size_t fa;
-    SampleState ss; FrameState fs; CondFrame tail;
-    std::vector<int> *fc; int cond_last; int deferred_fill; std::vector<float> *deferred; std::vector<int> *dfill;
+    int n, na, is_float, device;
+    StateCopy st;
+    std::vector<int> fc; int cond_last; int deferred_fill; std::vector<float> deferred; std::vector<int> dfill;
 };
+static Fields snapshot_fields(LPCNetB200Snapshot *s) { return state_fields(s->st.ss, s->st.fs, s->st.tail, s->n, s->na, s->is_float); }
 void lpcnet_b200_batch_snapshot_destroy(LPCNetB200Snapshot *s)
 {
     if (!s) return;
     cudaSetDevice(s->device);
-    free_sample_state(&s->ss);
-    free_frame_state(&s->fs);
-    void *ptrs[] = {s->tail.A, s->tail.B, s->tail.L};
-    for (void *p : ptrs) if (p) cudaFree(p);
-    delete s->fc; delete s->deferred; delete s->dfill;
-    free(s);
+    free_state(snapshot_fields(s));
+    delete s;
 }
 LPCNetB200Snapshot *lpcnet_b200_batch_snapshot_create(LPCNetB200Batch *b)
 {
     if (!b) { set_error("null batch"); return nullptr; }
     if (cudaSetDevice(b->device) != cudaSuccess) return nullptr;
-    LPCNetB200Snapshot *s = (LPCNetB200Snapshot *)calloc(1, sizeof(*s));
-    s->n = b->n; s->na = b->model.na; s->device = b->device; s->fa = condA_floats(b);
-    s->fc = new std::vector<int>(b->n, 0); s->deferred = new std::vector<float>(); s->dfill = new std::vector<int>(b->n, 0);
-    const size_t n = b->n;
-    bool ok = alloc_sample_state(&s->ss, n, s->na) == 0 && alloc_frame_state(&s->fs, n);
-    auto al = [&](void **p, size_t bytes) { if (ok && cudaMalloc(p, bytes) != cudaSuccess) ok = false; };
-    al((void **)&s->tail.A, sizeof(float) * s->fa); al((void **)&s->tail.B, sizeof(float) * n * 3 * NB); al((void **)&s->tail.L, sizeof(float) * n * LPC_ORDER);
-    if (!ok) { set_error("snapshot: device allocation failed"); lpcnet_b200_batch_snapshot_destroy(s); return nullptr; }
+    LPCNetB200Snapshot *s = new LPCNetB200Snapshot();
+    s->n = b->n; s->na = b->model.na; s->is_float = b->model.is_float; s->device = b->device;
+    s->fc.assign(b->n, 0); s->dfill.assign(b->n, 0);
+    if (!alloc_state(snapshot_fields(s), ALL)) { set_error("snapshot: device allocation failed"); lpcnet_b200_batch_snapshot_destroy(s); return nullptr; }
     return s;
 }
 static bool snapshot_fits(const LPCNetB200Batch *b, const LPCNetB200Snapshot *s)
 {
-    if (b && s && s->n == b->n && s->na == b->model.na && s->device == b->device && s->fa == condA_floats(b)) return true;
+    if (b && s && s->n == b->n && s->na == b->model.na && s->device == b->device && s->is_float == b->model.is_float) return true;
     set_error("snapshot does not belong to this batch");
     return false;
 }
@@ -1467,10 +1409,9 @@ int lpcnet_b200_batch_snapshot_save(LPCNetB200Batch *b, LPCNetB200Snapshot *s)
     if (!snapshot_fits(b, s)) return -1;
     CK(cudaSetDevice(b->device));
     if (order_enter(b, b->stream)) return -1;
-    if (copy_sample_state(s->ss, b->ss, b->n, s->na, b->stream) || copy_frame_state(s->fs, b->fs, b->n, b->stream)) return -1;
-    if (b->cond_last >= 0 && copy_cond_frame(b, s->tail, frame_at(b, b->cond_last), b->stream)) return -1;
+    if (copy_state(snapshot_fields(s), batch_fields(b, b->cond_last), b->cond_last >= 0 ? ALL : STATE, b->stream)) return -1;
     if (order_leave(b, b->stream)) return -1;
-    *s->fc = *b->fc; s->cond_last = b->cond_last; s->deferred_fill = b->deferred_fill; *s->deferred = *b->deferred; *s->dfill = *b->dfill;
+    s->fc = b->fc; s->cond_last = b->cond_last; s->deferred_fill = b->deferred_fill; s->deferred = b->deferred; s->dfill = b->dfill;
     return 0;
 }
 int lpcnet_b200_batch_snapshot_restore(LPCNetB200Batch *b, const LPCNetB200Snapshot *s)
@@ -1478,10 +1419,10 @@ int lpcnet_b200_batch_snapshot_restore(LPCNetB200Batch *b, const LPCNetB200Snaps
     if (!snapshot_fits(b, s)) return -1;
     CK(cudaSetDevice(b->device));
     if (order_enter(b, b->stream)) return -1;
-    if (copy_sample_state(b->ss, s->ss, b->n, s->na, b->stream) || copy_frame_state(b->fs, s->fs, b->n, b->stream)) return -1;
-    if (s->cond_last >= 0 && copy_cond_frame(b, frame_at(b, TAIL_SLOT), s->tail, b->stream)) return -1;
+    const Fields saved = snapshot_fields(const_cast<LPCNetB200Snapshot *>(s));
+    if (copy_state(batch_fields(b, TAIL_SLOT), saved, s->cond_last >= 0 ? ALL : STATE, b->stream)) return -1;
     if (order_leave(b, b->stream)) return -1;
-    *b->fc = *s->fc; b->deferred_fill = s->deferred_fill; *b->deferred = *s->deferred; *b->dfill = *s->dfill;
+    b->fc = s->fc; b->deferred_fill = s->deferred_fill; b->deferred = s->deferred; b->dfill = s->dfill;
     b->cond_last = s->cond_last >= 0 ? TAIL_SLOT : -1;
     return 0;
 }
@@ -1501,7 +1442,7 @@ int lpcnet_b200_debug_frame_network(LPCNetB200Batch *b, const float *features, i
     CK(cudaMemcpyAsync(b->d_features, features, fbytes, cudaMemcpyHostToDevice, b->stream));
     launch_frame_network(b->model, b->fs, b->d_features, (long long)nframes * feature_stride, feature_stride, n, nframes,
                          b->condA, b->condB, b->lpc_raw, b->stream);
-    for (int &v : *b->fc) v = std::min(1000, v + nframes);
+    for (int &v : b->fc) v = std::min(1000, v + nframes);
     b->cond_last = nframes - 1;
     const bool isf = b->model.is_float != 0;
     const size_t fA = condA_frame_floats(isf, n, na);

@@ -31,7 +31,7 @@ struct Shard {
 
 struct LPCNetB200Multi {
     int n;
-    std::vector<Shard> *shards;
+    std::vector<Shard> shards;
     bool peer_ok;                         // every device can write the memory of devices[0]
 };
 
@@ -61,18 +61,15 @@ int lpcnet_b200_shard_range(int n, int k, int parts, int *first, int *count)
 void lpcnet_b200_multi_destroy(LPCNetB200Multi *m)
 {
     if (!m) return;
-    if (m->shards) {
-        for (Shard &s : *m->shards) {
-            cudaSetDevice(s.device);
-            if (s.stream) cudaStreamSynchronize(s.stream);
-            if (s.batch) lpcnet_b200_batch_destroy(s.batch);
-            if (s.d_in) cudaFree(s.d_in);
-            if (s.d_pcm) cudaFree(s.d_pcm);
-            if (s.stream) cudaStreamDestroy(s.stream);
-        }
-        delete m->shards;
+    for (Shard &s : m->shards) {
+        cudaSetDevice(s.device);
+        if (s.stream) cudaStreamSynchronize(s.stream);
+        if (s.batch) lpcnet_b200_batch_destroy(s.batch);
+        if (s.d_in) cudaFree(s.d_in);
+        if (s.d_pcm) cudaFree(s.d_pcm);
+        if (s.stream) cudaStreamDestroy(s.stream);
     }
-    free(m);
+    delete m;
 }
 
 LPCNetB200Multi *lpcnet_b200_multi_create(int n_streams, const unsigned char *blob, int blob_len, const LPCNetB200Config *cfg,
@@ -87,16 +84,16 @@ LPCNetB200Multi *lpcnet_b200_multi_create(int n_streams, const unsigned char *bl
         if (d < 0 || d >= have) { set_error("multi_create: device %d out of range (%d devices)", d, have); return nullptr; }
         for (int j = 0; j < k; j++) if ((devices ? devices[j] : j) == d) { set_error("multi_create: device %d listed twice", d); return nullptr; }
     }
-    LPCNetB200Multi *m = (LPCNetB200Multi *)calloc(1, sizeof(*m));
-    m->n = n_streams; m->shards = new std::vector<Shard>(); m->peer_ok = true;
+    LPCNetB200Multi *m = new LPCNetB200Multi();
+    m->n = n_streams; m->peer_ok = true;
     for (int k = 0; k < n_devices; k++) {
         Shard s; memset(&s, 0, sizeof(s));
         s.device = devices ? devices[k] : k;
         lpcnet_b200_shard_range(n_streams, k, n_devices, &s.first, &s.count);
-        m->shards->push_back(s);
+        m->shards.push_back(s);
     }
-    const int dev0 = (*m->shards)[0].device;
-    for (Shard &s : *m->shards) {
+    const int dev0 = m->shards[0].device;
+    for (Shard &s : m->shards) {
         s.batch = lpcnet_b200_batch_create_ex(s.count, blob, blob_len, cfg, s.device);      // (sets the current device)
         if (!s.batch || cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) {
             if (s.batch) set_error("multi_create: stream creation failed on device %d", s.device);
@@ -113,13 +110,13 @@ LPCNetB200Multi *lpcnet_b200_multi_create(int n_streams, const unsigned char *bl
 }
 
 int lpcnet_b200_multi_streams(const LPCNetB200Multi *m) { return m ? m->n : 0; }
-int lpcnet_b200_multi_devices(const LPCNetB200Multi *m) { return m ? (int)m->shards->size() : 0; }
+int lpcnet_b200_multi_devices(const LPCNetB200Multi *m) { return m ? (int)m->shards.size() : 0; }
 int lpcnet_b200_multi_peer_access(const LPCNetB200Multi *m) { return m && m->peer_ok ? 1 : 0; }
 
 int lpcnet_b200_multi_shard(const LPCNetB200Multi *m, int k, int *device, int *first, int *count)
 {
-    if (!m || k < 0 || k >= (int)m->shards->size()) { set_error("multi_shard: bad shard index"); return -1; }
-    const Shard &s = (*m->shards)[k];
+    if (!m || k < 0 || k >= (int)m->shards.size()) { set_error("multi_shard: bad shard index"); return -1; }
+    const Shard &s = m->shards[k];
     if (device) *device = s.device;
     if (first) *first = s.first;
     if (count) *count = s.count;
@@ -128,20 +125,20 @@ int lpcnet_b200_multi_shard(const LPCNetB200Multi *m, int k, int *device, int *f
 // the shard's batch: per-stream lifecycle calls (reset_streams, export/import, snapshots ...) go through it with LOCAL stream ids
 LPCNetB200Batch *lpcnet_b200_multi_batch(LPCNetB200Multi *m, int k)
 {
-    if (!m || k < 0 || k >= (int)m->shards->size()) { set_error("multi_batch: bad shard index"); return nullptr; }
-    return (*m->shards)[k].batch;
+    if (!m || k < 0 || k >= (int)m->shards.size()) { set_error("multi_batch: bad shard index"); return nullptr; }
+    return m->shards[k].batch;
 }
 
 int lpcnet_b200_multi_reset(LPCNetB200Multi *m)
 {
     if (!m) { set_error("null multi-batch"); return -1; }
-    for (Shard &s : *m->shards) if (lpcnet_b200_batch_reset(s.batch)) return -1;
+    for (Shard &s : m->shards) if (lpcnet_b200_batch_reset(s.batch)) return -1;
     return 0;
 }
 int lpcnet_b200_multi_set_codebooks(LPCNetB200Multi *m, const float *cb, size_t n_floats)
 {
     if (!m) { set_error("null multi-batch"); return -1; }
-    for (Shard &s : *m->shards) if (lpcnet_b200_batch_set_codebooks(s.batch, cb, n_floats)) return -1;
+    for (Shard &s : m->shards) if (lpcnet_b200_batch_set_codebooks(s.batch, cb, n_floats)) return -1;
     return 0;
 }
 
@@ -153,7 +150,7 @@ static int run_all(LPCNetB200Multi *m, const void *in, size_t in_row_bytes, int 
     const long long T = decode ? (long long)units * 640 : (long long)units * spf;
     int rc = 0;
     // enqueue everything on every device first ...
-    for (Shard &s : *m->shards) {
+    for (Shard &s : m->shards) {
         CK(cudaSetDevice(s.device));
         const size_t ibytes = in_row_bytes * s.count, pbytes = sizeof(short) * (size_t)T * s.count;
         CK(cudaStreamSynchronize(s.stream));                                   // previous call's users of the staging buffers
@@ -166,7 +163,7 @@ static int run_all(LPCNetB200Multi *m, const void *in, size_t in_row_bytes, int 
         if (pcm_host) CK(cudaMemcpyAsync(pcm_host + (size_t)T * s.first, s.d_pcm, pbytes, cudaMemcpyDeviceToHost, s.stream));
     }
     // ... then wait for all of them (also on the error path: nothing may still be reading the caller's buffers)
-    for (Shard &s : *m->shards) {
+    for (Shard &s : m->shards) {
         cudaSetDevice(s.device);
         if (cudaStreamSynchronize(s.stream) != cudaSuccess && rc == 0) { set_error("multi: device %d: %s", s.device, cudaGetErrorString(cudaGetLastError())); rc = -1; }
     }
