@@ -274,6 +274,29 @@ LPCNET_EXPORT LPCNetB200EncBatch *lpcnet_b200_enc_create(int n_streams, int devi
 LPCNET_EXPORT void lpcnet_b200_enc_destroy(LPCNetB200EncBatch *e);
 LPCNET_EXPORT int lpcnet_b200_enc_reset(LPCNetB200EncBatch *e);                      /* lpcnet_encoder_init() for every stream */
 LPCNET_EXPORT int lpcnet_b200_enc_streams(const LPCNetB200EncBatch *e);
+/* == per-stream state ==  A row is its whole LPCNetEncState: analysis memory, pre-emphasis memory, pcount (the sub-frame slot),
+ * the pitch history, xc and frame weights, the excitation buffer, the Viterbi paths, best_i, vq_mem and the four-frame feature
+ * buffer.  What a row produces after a reset, an import or a copy equals, bit for bit, what the reference produces from that
+ * state, also for a row caught mid-superframe (pcount != 0 after single-frame calls).
+ * Every call below waits for all work queued on the batches it touches, on any CUDA stream, and returns when its work is
+ * complete; later calls on those batches, `_device` calls on caller streams included, are ordered after it.  Each returns -1
+ * (message: lpcnet_b200_last_error) and changes nothing for a NULL argument, count < 0 or a row out of range; count == 0 does
+ * nothing and succeeds. */
+/* lpcnet_encoder_init() for the listed streams only; the other streams carry on.  Ids may repeat. */
+LPCNET_EXPORT int lpcnet_b200_enc_reset_streams(LPCNetB200EncBatch *e, const int *streams, int count);
+/* One stream <-> opaque host blob of lpcnet_b200_enc_state_size() bytes: everything a later call reads.  An import validates
+ * the blob on the host first and refuses one whose pcount is outside 0..3 or whose best_i is outside 0..255. */
+LPCNET_EXPORT int lpcnet_b200_enc_state_size(const LPCNetB200EncBatch *e);
+LPCNET_EXPORT int lpcnet_b200_enc_export_state(LPCNetB200EncBatch *e, int stream, void *buf);
+LPCNET_EXPORT int lpcnet_b200_enc_import_state(LPCNetB200EncBatch *e, int stream, const void *buf);
+/* Row dst_rows[k] of dst becomes, bit for bit, what row src_rows[k] of src was before the call (compacting a batch whose
+ * sessions ended, moving a session to another batch or GPU, forking one).  The source is unchanged; src == dst is allowed and
+ * every read sees the state from before the call (a rotation of rows works); source rows may repeat (cloning); destination
+ * rows must be distinct (a repeated one is refused like a row out of range).  Rows not listed are untouched.  Codebooks are
+ * not compared: a copied row goes on under dst's codebooks, and dst without codebooks still refuses _encode.  src and dst may
+ * be on different devices of this process (peer DMA when the devices allow it, staged by the driver otherwise). */
+LPCNET_EXPORT int lpcnet_b200_enc_copy_streams(LPCNetB200EncBatch *dst, const int *dst_rows,
+                                               LPCNetB200EncBatch *src, const int *src_rows, int count);
 /* the VQ codebooks lpcnet_encode searches (same four arrays, same order as lpcnet_b200_batch_set_codebooks) */
 LPCNET_EXPORT int lpcnet_b200_enc_set_codebooks(LPCNetB200EncBatch *e, const float *cb, size_t n_floats);
 /* == lpcnet_compute_single_frame_features() per stream and frame (src/lpcnet_enc.c:919; `lpcnet_demo -features`) ==

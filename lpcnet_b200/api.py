@@ -131,6 +131,11 @@ def lib():
     L.lpcnet_b200_enc_destroy.argtypes = [c_p]
     L.lpcnet_b200_enc_reset.argtypes = [c_p]
     L.lpcnet_b200_enc_streams.argtypes = [c_p]
+    L.lpcnet_b200_enc_reset_streams.argtypes = [c_p, c_p, ctypes.c_int]
+    L.lpcnet_b200_enc_state_size.argtypes = [c_p]
+    L.lpcnet_b200_enc_export_state.argtypes = [c_p, ctypes.c_int, c_p]
+    L.lpcnet_b200_enc_import_state.argtypes = [c_p, ctypes.c_int, c_p]
+    L.lpcnet_b200_enc_copy_streams.argtypes = [c_p, c_p, c_p, c_p, ctypes.c_int]
     L.lpcnet_b200_enc_set_codebooks.argtypes = [c_p, c_p, ctypes.c_size_t]
     L.lpcnet_b200_enc_compute_features.argtypes = [c_p, c_p, ctypes.c_int, c_p]
     L.lpcnet_b200_enc_compute_features_float.argtypes = [c_p, c_p, ctypes.c_int, c_p]
@@ -336,6 +341,38 @@ class EncBatch:
     def reset(self):
         if self._L.lpcnet_b200_enc_reset(self._h) != 0:
             raise LPCNetB200Error(_err())
+
+    def reset_streams(self, streams):
+        """lpcnet_encoder_init for the listed streams only (ids may repeat); the others carry on."""
+        ids = np.ascontiguousarray(streams, dtype=np.int32)
+        if self._L.lpcnet_b200_enc_reset_streams(self._h, ids.ctypes.data, int(ids.size)) != 0:
+            raise LPCNetB200Error(_err())
+
+    def state_size(self):
+        return int(self._L.lpcnet_b200_enc_state_size(self._h))
+
+    def export_state(self, s):
+        """stream s's whole analysis state as an opaque uint8 blob of state_size() bytes"""
+        buf = np.zeros(self.state_size(), dtype=np.uint8)
+        if self._L.lpcnet_b200_enc_export_state(self._h, int(s), buf.ctypes.data) != 0:
+            raise LPCNetB200Error(_err())
+        return buf
+
+    def import_state(self, s, buf):
+        b = np.ascontiguousarray(buf).view(np.uint8).ravel()
+        assert b.size == self.state_size()
+        if self._L.lpcnet_b200_enc_import_state(self._h, int(s), b.ctypes.data) != 0:
+            raise LPCNetB200Error(_err())
+
+    def copy_streams(self, dst_rows, src_enc_batch, src_rows):
+        """Row dst_rows[k] of this batch becomes what row src_rows[k] of src_enc_batch (this batch allowed) was before the call,
+        copied on the device (lpcnet_b200_enc_copy_streams)."""
+        d = np.ascontiguousarray(dst_rows, dtype=np.int32)
+        s = np.ascontiguousarray(src_rows, dtype=np.int32)
+        if d.shape != s.shape:
+            raise LPCNetB200Error("copy_streams: %d destination rows for %d source rows" % (d.size, s.size))
+        if self._L.lpcnet_b200_enc_copy_streams(self._h, d.ctypes.data, src_enc_batch._h, s.ctypes.data, int(d.size)) != 0:
+            raise LPCNetB200Error("copy_streams: " + _err())
 
     def compute_features(self, pcm):
         """pcm [n][T*160] int16 (or float32: the _float entry point) -> features [n][T][36]."""

@@ -17,6 +17,8 @@
 // features and the packets equal the reference's bit for bit; the independent pieces (window, FFT butterflies, bands, the
 // 256 lags of the pitch correlation, Viterbi states, codebook distances) are dealt to the threads.
 // The three libm calls in double (log10 :516, log :676, pow freq.c:318) use CUDA's double routines.
+#include <algorithm>
+#include <cstddef>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -616,6 +618,18 @@ __global__ void __launch_bounds__(ENC_THREADS, 4) enc_kernel(const EncArgs a)
     }
 }
 
+// Whole rows of [rows][ENC_STATE_WORDS] arrays (per-stream resets, export / import, copies between batches): block k writes row
+// dst_rows[k] of dst from row src_rows[k] of src (a NULL row list: row k, i.e. the k-th record of a staging buffer; src == NULL:
+// zeros, lpcnet_encoder_init).  A row is 4011 words and rows are only 4-byte aligned, so the copy goes word by word, consecutive
+// threads on consecutive words.
+__global__ void __launch_bounds__(ENC_THREADS) enc_rows_kernel(uint32_t *dst, const int *dst_rows, const uint32_t *src, const int *src_rows)
+{
+    const int k = blockIdx.x;
+    uint32_t *d = dst + (size_t)(dst_rows ? dst_rows[k] : k) * ENC_STATE_WORDS;
+    const uint32_t *s = src ? src + (size_t)(src_rows ? src_rows[k] : k) * ENC_STATE_WORDS : nullptr;
+    for (int i = threadIdx.x; i < ENC_STATE_WORDS; i += ENC_THREADS) d[i] = s ? s[i] : 0u;
+}
+
 }  // namespace lpcnet_b200
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -796,6 +810,137 @@ int lpcnet_b200_enc_encode_device(LPCNetB200EncBatch *e, const short *d_pcm, int
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : e->stream;
     if (enc_run_device(e, 1, d_pcm, nullptr, npackets, nullptr, d_packets, st)) return -1;
     if (!cuda_stream) CK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// ---- per-stream state: resets, state by value, copies between batches (the reference copies LPCNetEncState by value) ----
+// A row is its whole EncState.  Every call below runs on the batch's own stream after everything queued on the batches it
+// touches (enc_order_enter) and returns when its work is complete.  Staging reuses the buffers of the host-pointer calls,
+// grown on demand and kept at the largest size used: d_in holds the row lists (2 x count ints), d_out the packed records
+// (count x 16,044 bytes for a copy inside one batch or across devices, 66 MB for 4096 rows; one record for export / import).
+// A copy between two batches of one device needs no record staging.
+static_assert(sizeof(EncState) == 16044, "the exported record is one EncState");
+
+static int enc_rows_check(const LPCNetB200EncBatch *e, const int *rows, int count, bool distinct, const char *what)
+{
+    std::vector<char> seen(distinct ? e->n : 0, 0);
+    for (int k = 0; k < count; k++) {
+        if (rows[k] < 0 || rows[k] >= e->n) { set_error("%s row %d out of range (%d streams)", what, rows[k], e->n); return -1; }
+        if (distinct && seen[rows[k]]) { set_error("%s row %d listed twice", what, rows[k]); return -1; }
+        if (distinct) seen[rows[k]] = 1;
+    }
+    return 0;
+}
+
+int lpcnet_b200_enc_reset_streams(LPCNetB200EncBatch *e, const int *streams, int count)
+{
+    if (!e || !streams || count < 0) { set_error("enc_reset_streams: bad arguments"); return -1; }
+    if (enc_rows_check(e, streams, count, false, "enc_reset_streams: stream")) return -1;
+    if (count == 0) return 0;
+    CK(cudaSetDevice(e->device));
+    if (enc_grow(&e->d_in, &e->d_in_cap, sizeof(int) * (size_t)count)) return -1;
+    if (enc_order_enter(e, e->stream)) return -1;
+    CK(cudaMemcpyAsync(e->d_in, streams, sizeof(int) * (size_t)count, cudaMemcpyHostToDevice, e->stream));
+    enc_rows_kernel<<<count, ENC_THREADS, 0, e->stream>>>(reinterpret_cast<uint32_t *>(e->state), (const int *)e->d_in, nullptr, nullptr);
+    CK(cudaGetLastError());
+    if (enc_order_leave(e, e->stream)) return -1;
+    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+
+int lpcnet_b200_enc_state_size(const LPCNetB200EncBatch *e) { return e ? (int)sizeof(EncState) : -1; }
+
+// row s <-> host record `buf` through d_out: the one-row use of a copy's pack and unpack
+static int enc_state_move(LPCNetB200EncBatch *e, int s, void *buf, bool unpack)
+{
+    CK(cudaSetDevice(e->device));
+    if (enc_grow(&e->d_out, &e->d_out_cap, sizeof(EncState))) return -1;
+    uint32_t *row = reinterpret_cast<uint32_t *>(e->state + s), *rec = (uint32_t *)e->d_out;
+    if (enc_order_enter(e, e->stream)) return -1;
+    if (unpack) {
+        CK(cudaMemcpyAsync(rec, buf, sizeof(EncState), cudaMemcpyHostToDevice, e->stream));
+        enc_rows_kernel<<<1, ENC_THREADS, 0, e->stream>>>(row, nullptr, rec, nullptr);
+    } else {
+        enc_rows_kernel<<<1, ENC_THREADS, 0, e->stream>>>(rec, nullptr, row, nullptr);
+        CK(cudaMemcpyAsync(buf, rec, sizeof(EncState), cudaMemcpyDeviceToHost, e->stream));
+    }
+    CK(cudaGetLastError());
+    if (enc_order_leave(e, e->stream)) return -1;
+    CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+
+int lpcnet_b200_enc_export_state(LPCNetB200EncBatch *e, int s, void *buf)
+{
+    if (!e || !buf || s < 0 || s >= e->n) { set_error("enc_export_state: bad arguments"); return -1; }
+    return enc_state_move(e, s, buf, false);
+}
+
+int lpcnet_b200_enc_import_state(LPCNetB200EncBatch *e, int s, const void *buf)
+{
+    if (!e || !buf || s < 0 || s >= e->n) { set_error("enc_import_state: bad arguments"); return -1; }
+    // pcount and best_i index the kernel's shared-memory arrays (features[pcount], xc[2 + 2 * pcount + sub], xc[..][best_i],
+    // pitch_prev[..][best_i]): a record that would take them out of range never reaches the device
+    int pcount, best_i;
+    memcpy(&pcount, (const char *)buf + offsetof(EncState, pcount), sizeof(int));
+    memcpy(&best_i, (const char *)buf + offsetof(EncState, best_i), sizeof(int));
+    if (pcount < 0 || pcount > 3) { set_error("enc_import_state: pcount %d outside 0..3", pcount); return -1; }
+    if (best_i < 0 || best_i >= PMAX) { set_error("enc_import_state: best_i %d outside 0..%d", best_i, PMAX - 1); return -1; }
+    return enc_state_move(e, s, const_cast<void *>(buf), true);
+}
+
+// Rows of src into rows of dst.  Between two batches of one device: one kernel, row to row, on dst's stream.  Inside one batch
+// (every record is read before any is written, so a rotation works) and across devices: the records are packed into src's
+// staging on src's stream, copied into dst's staging (peer DMA across devices) and unpacked on dst's stream.
+int lpcnet_b200_enc_copy_streams(LPCNetB200EncBatch *dst, const int *dst_rows, LPCNetB200EncBatch *src, const int *src_rows, int count)
+{
+    if (!dst || !dst_rows || !src || !src_rows || count < 0) { set_error("enc_copy_streams: bad arguments"); return -1; }
+    if (enc_rows_check(src, src_rows, count, false, "enc_copy_streams: source") ||
+        enc_rows_check(dst, dst_rows, count, true, "enc_copy_streams: destination")) return -1;
+    if (count == 0) return 0;
+    const size_t rows_bytes = sizeof(int) * 2 * (size_t)count, rec_bytes = sizeof(EncState) * (size_t)count;
+    std::vector<int> rows(2 * (size_t)count);                      // the source rows, then the destination rows
+    std::copy(src_rows, src_rows + count, rows.begin());
+    std::copy(dst_rows, dst_rows + count, rows.begin() + count);
+    uint32_t *s_state = reinterpret_cast<uint32_t *>(src->state), *d_state = reinterpret_cast<uint32_t *>(dst->state);
+    if (src != dst && src->device == dst->device) {
+        CK(cudaSetDevice(dst->device));
+        if (enc_grow(&dst->d_in, &dst->d_in_cap, rows_bytes)) return -1;
+        const int *d_rows = (const int *)dst->d_in;
+        if (enc_order_enter(dst, dst->stream)) return -1;
+        if (src->has_order) CK(cudaStreamWaitEvent(dst->stream, src->order_ev, 0));
+        CK(cudaMemcpyAsync(dst->d_in, rows.data(), rows_bytes, cudaMemcpyHostToDevice, dst->stream));
+        enc_rows_kernel<<<count, ENC_THREADS, 0, dst->stream>>>(d_state, d_rows + count, s_state, d_rows);
+        CK(cudaGetLastError());
+        if (enc_order_leave(dst, dst->stream)) return -1;
+        CK(cudaStreamSynchronize(dst->stream));
+        return 0;
+    }
+    CK(cudaSetDevice(src->device));
+    if (enc_grow(&src->d_in, &src->d_in_cap, rows_bytes) || enc_grow(&src->d_out, &src->d_out_cap, rec_bytes)) return -1;
+    CK(cudaSetDevice(dst->device));
+    if (dst != src && (enc_grow(&dst->d_in, &dst->d_in_cap, rows_bytes) || enc_grow(&dst->d_out, &dst->d_out_cap, rec_bytes))) return -1;
+    // 1. pack on src's stream; src's order event marks the records ready
+    CK(cudaSetDevice(src->device));
+    if (enc_order_enter(src, src->stream)) return -1;
+    CK(cudaMemcpyAsync(src->d_in, rows.data(), rows_bytes, cudaMemcpyHostToDevice, src->stream));
+    enc_rows_kernel<<<count, ENC_THREADS, 0, src->stream>>>((uint32_t *)src->d_out, nullptr, s_state, (const int *)src->d_in);
+    CK(cudaGetLastError());
+    if (enc_order_leave(src, src->stream)) return -1;
+    // 2. dst's stream waits for it (and for dst's own last call), takes the records and unpacks them
+    CK(cudaSetDevice(dst->device));
+    if (enc_order_enter(dst, dst->stream)) return -1;
+    if (dst != src) {
+        CK(cudaStreamWaitEvent(dst->stream, src->order_ev, 0));
+        CK(cudaMemcpyAsync(dst->d_in, rows.data(), rows_bytes, cudaMemcpyHostToDevice, dst->stream));
+        CK(cudaMemcpyPeerAsync(dst->d_out, dst->device, src->d_out, src->device, rec_bytes, dst->stream));
+    }
+    enc_rows_kernel<<<count, ENC_THREADS, 0, dst->stream>>>(d_state, (const int *)dst->d_in + count, (const uint32_t *)dst->d_out, nullptr);
+    CK(cudaGetLastError());
+    if (enc_order_leave(dst, dst->stream)) return -1;
+    CK(cudaStreamSynchronize(dst->stream));
+    CK(cudaSetDevice(src->device));
+    CK(cudaStreamSynchronize(src->stream));
     return 0;
 }
 
