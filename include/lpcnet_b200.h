@@ -231,8 +231,8 @@ LPCNET_EXPORT int lpcnet_b200_batch_decode_device(LPCNetB200Batch *b, const unsi
                                                   short *d_pcm, void *cuda_stream);
 
 /* == groups: several batches of one model shape in one per-sample launch ==
- * Several existing batches on ONE device with the same GRU_A size, all int8, each at most once (at most 16): their
- * synthesize / decode calls run as one.  Each member runs its own frame network and its own silent-frame launches, then every
+ * Several existing batches on ONE device with the same GRU_A size and one flavour (all int8 or all float), each at most once
+ * (at most 16): their synthesize / decode calls run as one.  Each member runs its own frame network and its own silent-frame launches, then every
  * member's remaining frames take ONE per-sample kernel launch that spreads all members' streams over the SMs together (no
  * CTA holds streams of two members).  Group stream g = the streams of batches[0], then batches[1], ... in order (the sum of
  * their sizes); features, packets and PCM are laid out as for a batch of that many streams.
@@ -242,8 +242,11 @@ LPCNET_EXPORT int lpcnet_b200_batch_decode_device(LPCNetB200Batch *b, const unsi
  * which keep their own switches (FEATURES_DELAY, END2END, LPC_GAMMA) and sparsity patterns.  Group calls are ordered with
  * the members' own calls like any other call, so `_device` group calls may be mixed with member calls on any stream.
  * A member with a PCM sink set is refused.  The group does not own its members: destroy the group before any member.
+ * Float groups pick their kernel as a float batch does: the neuron-per-lane kernel while the plan's streams per CTA is at most
+ * 4, the lane == stream kernel above that (or always, with LPCNET_B200_FLOAT_LANE_STREAM set at create).
  * group_create returns NULL (message: lpcnet_b200_last_error) for members on different devices, with different GRU_A
- * sizes, a float member, a member listed twice, or more than 16 members.  LPCNET_B200_STREAMS_PER_CTA is read at create. */
+ * sizes, int8 and float members mixed, a member listed twice, or more than 16 members.  LPCNET_B200_STREAMS_PER_CTA is read
+ * at create. */
 typedef struct LPCNetB200Group LPCNetB200Group;
 LPCNET_EXPORT LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int count);
 LPCNET_EXPORT void lpcnet_b200_group_destroy(LPCNetB200Group *g);
@@ -264,6 +267,13 @@ LPCNET_EXPORT float lpcnet_b200_group_last_sample_kernel_ms(const LPCNetB200Grou
  * per CTA (1..32) for which sum ceil(n[k] / spc) <= sms, 32 if none; override_spc > 0 pins it (LPCNET_B200_STREAMS_PER_CTA).
  * Member k takes ceil(n[k] / spc) consecutive CTAs; *ctas = their total.  spc <= 16 selects the half-A-only schedule. */
 LPCNET_EXPORT int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_spc, int *spc, int *ctas);
+/* Test hook (host only, no CUDA): the launch plan of a float group.  *spc as above; then, as for a float batch, spc <= 4 with
+ * lane_stream 0 selects the neuron-per-lane kernel, whose CTAs lay out *slots = 1, 2 or 4 streams (spc 3 -> 4), and anything
+ * else the lane == stream kernel with *slots = spc.  Member k takes ceil(n[k] / slots) consecutive CTAs; *ctas = their total.
+ * lane_stream != 0 stands for LPCNET_B200_FLOAT_LANE_STREAM.  Returns 1 for the neuron-per-lane kernel, 0 for the lane == stream
+ * kernel, -1 for bad arguments. */
+LPCNET_EXPORT int lpcnet_b200_debug_group_plan_float(const int *n, int count, int sms, int override_spc, int lane_stream,
+                                                     int *spc, int *slots, int *ctas);
 
 /* == the analysis side, batched (SURVEY 8f N2): feature extraction and the 1.6 kb/s encoder ==
  * n independent LPCNetEncState streams (reference src/lpcnet_private.h:55-75) on one device, all starting from

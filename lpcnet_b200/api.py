@@ -77,6 +77,7 @@ def lib():
     L.lpcnet_b200_group_last_sample_kernel_ms.restype = ctypes.c_float
     L.lpcnet_b200_group_last_sample_kernel_ms.argtypes = [c_p, c_p]
     L.lpcnet_b200_debug_group_plan.argtypes = [c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p]
+    L.lpcnet_b200_debug_group_plan_float.argtypes = [c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
     L.lpcnet_b200_batch_is_float.argtypes = [c_p]
     L.lpcnet_b200_batch_get_state.argtypes = [c_p, ctypes.c_int, c_p, c_p, c_p, c_p, c_p]
     L.lpcnet_b200_debug_frame_network.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
@@ -633,9 +634,23 @@ def group_plan(sizes, sms, override_spc=0):
     return int(spc.value), int(ctas.value)
 
 
+def group_plan_float(sizes, sms, override_spc=0, lane_stream=False):
+    """Launch plan of a float group whose members have `sizes` streams on `sms` SMs: (kernel, streams per CTA, slots, CTA count),
+    kernel "neuron" (neuron-per-lane, `slots` = 1, 2 or 4 streams per CTA) or "lane" (lane == stream, slots = spc);
+    lane_stream stands for LPCNET_B200_FLOAT_LANE_STREAM (lpcnet_b200_debug_group_plan_float; host only, needs no GPU)."""
+    n = (ctypes.c_int * len(sizes))(*[int(v) for v in sizes])
+    spc, slots, ctas = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int(0)
+    r = lib().lpcnet_b200_debug_group_plan_float(n, len(sizes), int(sms), int(override_spc), int(bool(lane_stream)),
+                                                 ctypes.byref(spc), ctypes.byref(slots), ctypes.byref(ctas))
+    if r < 0:
+        raise LPCNetB200Error("debug_group_plan_float: " + _err())
+    return ("neuron" if r == 1 else "lane"), int(spc.value), int(slots.value), int(ctas.value)
+
+
 class Group:
-    """The synthesize / decode calls of several int8 Batch objects of one GRU_A size on one device as one call: one per-sample
-    launch for all their streams (lpcnet_b200_group_*).  Group stream rows = batches[0]'s streams, then batches[1]'s, ...
+    """The synthesize / decode calls of several Batch objects of one flavour (all int8 or all float) and one GRU_A size on one
+    device as one call: one per-sample launch for all their streams (lpcnet_b200_group_*).  Group stream rows = batches[0]'s
+    streams, then batches[1]'s, ...
     The members stay usable on their own; the group keeps them alive and must be closed before they are."""
 
     def __init__(self, batches):

@@ -827,14 +827,17 @@ float lpcnet_b200_batch_last_sample_kernel_ms(const LPCNetB200Batch *b, int *lau
     return timed_ms(b->kev, b->kev_used);
 }
 
-// ---- groups: the synthesize / decode calls of several int8 batches of one GRU_A size on one device as one call ----
+// ---- groups: the synthesize / decode calls of several batches of one flavour and GRU_A size on one device as one call ----
 // Each chunk runs every member's 100 Hz part and silent-frame prefix with the member's own launches, then ONE per-sample launch
-// for the frames that remain (GroupSampleParams, sample_kernel.cu).  The members keep all their state and host mirrors; the
-// group only holds the launch plan, a stream for its host-pointer calls and the event timers of its launches.
+// for the frames that remain (GroupSampleParams; sample_kernel.cu, sample_kernel_f32.cu, sample_kernel_f32n.cu).  The members
+// keep all their state and host mirrors; the group only holds the launch plan, a stream for its host-pointer calls and the event
+// timers of its launches.
 struct LPCNetB200Group {
     int count, device, na, n_total;
     LPCNetB200Batch *m[GROUP_MAX];
-    int spc, ctas;                    // the launch plan (group_plan)
+    bool is_float;                    // the members' flavour
+    bool neuron;                      // float: the neuron-per-lane kernel (group_plan_float)
+    int spc, slots, ctas;             // the launch plan (group_plan, group_plan_float): slots = streams a CTA lays out
     bool fast_cvt;                    // conversion-free rounding: only if every member allows it
     uint32_t smem_bytes;              // largest shared-memory footprint of the members
     cudaStream_t stream;
@@ -862,6 +865,26 @@ int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_
     return 0;
 }
 
+// The float flavour takes spc from group_plan and then the kernel a batch would (launch_sample): at spc <= FN_S, unless
+// LPCNET_B200_FLOAT_LANE_STREAM is set, the neuron-per-lane kernel, whose CTAs lay out S = 1, 2 or FN_S streams (spc 3 -> 4);
+// otherwise the lane == stream kernel with spc.  Member k takes ceil(n_k / slots) CTAs.  Returns true for the neuron-per-lane kernel.
+static bool group_plan_float(const int *n, int count, int sms, int override_spc, bool lane_stream, int *spc, int *slots, int *ctas)
+{
+    *spc = group_plan(n, count, sms, override_spc, ctas);
+    const bool neuron = *spc <= FN_S && !lane_stream;
+    *slots = !neuron ? *spc : *spc <= 1 ? 1 : *spc == 2 ? 2 : FN_S;
+    *ctas = 0;
+    for (int k = 0; k < count; k++) *ctas += (n[k] + *slots - 1) / *slots;
+    return neuron;
+}
+
+int lpcnet_b200_debug_group_plan_float(const int *n, int count, int sms, int override_spc, int lane_stream, int *spc, int *slots, int *ctas)
+{
+    if (!n || count < 1 || count > GROUP_MAX || sms < 1 || !spc || !slots || !ctas) { set_error("debug_group_plan_float: bad arguments"); return -1; }
+    for (int k = 0; k < count; k++) if (n[k] < 1) { set_error("debug_group_plan_float: member %d has no streams", k); return -1; }
+    return group_plan_float(n, count, sms, override_spc, lane_stream != 0, spc, slots, ctas) ? 1 : 0;
+}
+
 void lpcnet_b200_group_destroy(LPCNetB200Group *g)
 {
     if (!g) return;
@@ -877,7 +900,11 @@ LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int c
     for (int k = 0; k < count; k++) {
         const LPCNetB200Batch *b = batches[k];
         if (!b) { set_error("group_create: member %d is NULL", k); return nullptr; }
-        if (b->model.is_float) { set_error("group_create: member %d holds a float model; groups run int8 models only", k); return nullptr; }
+        if (b->model.is_float != batches[0]->model.is_float) {
+            set_error("group_create: member %d holds %s model, member 0 %s one; the members of a group are all int8 or all float", k,
+                      b->model.is_float ? "a float" : "an int8", batches[0]->model.is_float ? "a float" : "an int8");
+            return nullptr;
+        }
         if (b->device != batches[0]->device) { set_error("group_create: member %d is on device %d, member 0 on device %d", k, b->device, batches[0]->device); return nullptr; }
         if (b->model.na != batches[0]->model.na) { set_error("group_create: member %d has %d GRU_A units, member 0 has %d", k, b->model.na, batches[0]->model.na); return nullptr; }
         for (int j = 0; j < k; j++) if (batches[j] == b) { set_error("group_create: member %d is listed twice (also member %d)", k, j); return nullptr; }
@@ -885,18 +912,25 @@ LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int c
     if (cudaSetDevice(batches[0]->device) != cudaSuccess) { set_error("group_create: cudaSetDevice(%d) failed", batches[0]->device); return nullptr; }
     LPCNetB200Group *g = new LPCNetB200Group();
     g->count = count; g->device = batches[0]->device; g->na = batches[0]->model.na;
+    g->is_float = batches[0]->model.is_float != 0;
     g->fast_cvt = true;
     int n[GROUP_MAX];
     for (int k = 0; k < count; k++) {
         LPCNetB200Batch *b = batches[k];
         g->m[k] = b; n[k] = b->n; g->n_total += b->n;
         g->fast_cvt = g->fast_cvt && batch_fast_cvt(b);
-        g->smem_bytes = std::max(g->smem_bytes, b->model.L.total_bytes);
     }
     int dev = g->device, sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     const char *e = getenv("LPCNET_B200_STREAMS_PER_CTA");
-    g->spc = group_plan(n, count, sms, e ? atoi(e) : 0, &g->ctas);
+    if (g->is_float) {
+        g->neuron = group_plan_float(n, count, sms, e ? atoi(e) : 0, getenv("LPCNET_B200_FLOAT_LANE_STREAM") != nullptr, &g->spc, &g->slots, &g->ctas);
+    } else {
+        g->spc = group_plan(n, count, sms, e ? atoi(e) : 0, &g->ctas);
+        g->slots = g->spc;
+    }
+    for (int k = 0; k < count; k++)      // the footprint of the layout the chosen kernel uses
+        g->smem_bytes = std::max(g->smem_bytes, g->neuron ? batches[k]->model.Ln.total_bytes : batches[k]->model.L.total_bytes);
     if (cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) != cudaSuccess) {
         set_error("group_create: cudaStreamCreate failed"); lpcnet_b200_group_destroy(g); return nullptr;
     }
@@ -918,17 +952,22 @@ static int launch_group(LPCNetB200Group *g, const int *live0, int nf, int spf, s
         p.spc = g->spc;
         p.one_half = g->spc <= HALF;
         p.fast_cvt = g->fast_cvt ? 1 : 0;
+        if (g->neuron) { p.L = b->model.Ln; p.image = b->model.image_n; }     // the member's neuron-per-lane layout and image
         gp.cta0[gp.count++] = ctas;
-        ctas += (b->n + g->spc - 1) / g->spc;
+        ctas += (b->n + g->slots - 1) / g->slots;
     }
     if (!gp.count) return 0;
     if (time_launch(g->kev, &g->kev_used, st)) return -1;
     cudaError_t e;
+#define LPCNET_GROUP_DISPATCH(ns) (!g->is_float ? ns::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st) \
+                                   : g->neuron ? ns::launch_group_sample_kernel_f32n(gp, ctas, g->smem_bytes, st) \
+                                               : ns::launch_group_sample_kernel_f32(gp, ctas, g->smem_bytes, st))
     switch (g->na) {
-    case 128: e = na128::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st); break;
-    case 256: e = na256::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st); break;
-    default:  e = na384::launch_group_sample_kernel(gp, ctas, g->smem_bytes, st); break;
+    case 128: e = LPCNET_GROUP_DISPATCH(na128); break;
+    case 256: e = LPCNET_GROUP_DISPATCH(na256); break;
+    default:  e = LPCNET_GROUP_DISPATCH(na384); break;
     }
+#undef LPCNET_GROUP_DISPATCH
     if (e != cudaSuccess) { set_error("group per-sample kernel launch failed: %s", cudaGetErrorString(e)); return -1; }
     if (time_launch(g->kev, &g->kev_used, st)) return -1;
     return 1;

@@ -348,9 +348,10 @@ struct SampleParams {
 // (the layout of SampleParams is kept as it is: one more word made the int8 kernel slower; new per-call switches
 // are packed into existing words)
 
-// One per-sample launch over the batches of a group (lpcnet_b200_group_*, int8 only): member k's streams are CTAs
-// [cta0[k], cta0[k] + ceil(n_k / spc)) of the grid, every CTA holds streams of one member only.  spc, one_half and fast_cvt are
-// the group's and the same in every m[k].
+// One per-sample launch over the batches of a group (lpcnet_b200_group_*, all int8 or all float): member k's streams are CTAs
+// [cta0[k], cta0[k] + ceil(n_k / slots)) of the grid, every CTA holds streams of one member only.  slots = spc, except in the
+// neuron-per-lane float kernel, whose CTAs lay out S = 1, 2 or FN_S streams (spc 3 -> S 4).  spc, one_half and fast_cvt are the
+// group's and the same in every m[k].
 constexpr int GROUP_MAX = 16;        // members of a group: GROUP_MAX SampleParams fill most of the 4 KB of kernel parameters
 struct GroupSampleParams {
     SampleParams m[GROUP_MAX];
@@ -394,7 +395,9 @@ void launch_decode_packets(const DeviceModel &m, const FrameState &fs, const uin
     cudaError_t launch_sample_kernel(const SampleParams &p, cudaStream_t st); \
     cudaError_t launch_sample_kernel_f32(const SampleParams &p, cudaStream_t st); \
     cudaError_t launch_sample_kernel_f32n(const SampleParams &p, cudaStream_t st);   /* p.L / p.image = DeviceModel::Ln / image_n, p.spc <= FN_S */ \
-    cudaError_t launch_group_sample_kernel(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st); }
+    cudaError_t launch_group_sample_kernel(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st); \
+    cudaError_t launch_group_sample_kernel_f32(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st); \
+    cudaError_t launch_group_sample_kernel_f32n(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st);   /* S from m[0].spc <= FN_S */ }
 LPCNET_DECLARE_LAUNCHERS(na128)
 LPCNET_DECLARE_LAUNCHERS(na256)
 LPCNET_DECLARE_LAUNCHERS(na384)

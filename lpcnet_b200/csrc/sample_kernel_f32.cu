@@ -65,13 +65,15 @@ __device__ __forceinline__ void gemv_f32(float y[8], const uint8_t *__restrict__
 
 }  // namespace
 
-__global__ void __launch_bounds__(F_THREADS, 1) lpcnet_sample_kernel_f32(const __grid_constant__ SampleParams P)
+// The body of the kernel for the streams of `P` that CTA `cta` of their batch holds.  A single-batch launch runs it with its own
+// parameters and blockIdx.x; a group launch with the parameters of the CTA's member and the member-local CTA index.
+__device__ __forceinline__ void sample_body_f32(const SampleParams &P, int cta)
 {
     extern __shared__ __align__(128) uint8_t smem[];
     const SmemLayout &L = P.L;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n = P.n_streams;
-    const int s_raw = blockIdx.x * P.spc + lane;                 // lanes >= spc are dead slots (shadow the last stream, stores masked)
+    const int s_raw = cta * P.spc + lane;                        // lanes >= spc are dead slots (shadow the last stream, stores masked)
     const bool live = lane < P.spc && s_raw < n;
     const int s = live ? s_raw : n - 1;
 
@@ -288,6 +290,31 @@ __global__ void __launch_bounds__(F_THREADS, 1) lpcnet_sample_kernel_f32(const _
             P.rng[s] = rng.z; P.rng[(size_t)n + s] = rng.w; P.rng[2 * (size_t)n + s] = rng.jsr; P.rng[3 * (size_t)n + s] = rng.jcong;
         }
     }
+}
+
+__global__ void __launch_bounds__(F_THREADS, 1) lpcnet_sample_kernel_f32(const __grid_constant__ SampleParams P)
+{
+    sample_body_f32(P, blockIdx.x);
+}
+
+// Several float batches of one GRU_A size in one launch: member k holds CTAs [cta0[k], cta0[k+1]) (GroupSampleParams, engine.h),
+// spc live slots each.  Everything that differs between members (image, layout, the dense GRU_B flag, stream count) is read from
+// the member's parameters, so members with different sparsity patterns share the launch.
+__global__ void __launch_bounds__(F_THREADS, 1) lpcnet_group_sample_kernel_f32(const __grid_constant__ GroupSampleParams G)
+{
+    const int c = blockIdx.x;
+    int k = 0;
+#pragma unroll 1
+    for (int j = 1; j < G.count; j++) if (c >= G.cta0[j]) k = j;
+    sample_body_f32(G.m[k], c - G.cta0[k]);
+}
+
+cudaError_t launch_group_sample_kernel_f32(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st)
+{
+    cudaError_t e = cudaFuncSetAttribute(lpcnet_group_sample_kernel_f32, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    lpcnet_group_sample_kernel_f32<<<ctas, F_THREADS, smem_bytes, st>>>(g);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_sample_kernel_f32(const SampleParams &p, cudaStream_t st)

@@ -74,13 +74,15 @@ __device__ __forceinline__ void chain(float (&y)[FN_S], const uint8_t *__restric
     }
 }
 
+// the streams of `P` that CTA `cta` of their batch holds: blockIdx.x in a single-batch launch, the member-local CTA index in a
+// group launch
 template <int S>
-__device__ __forceinline__ void run(const SampleParams &P, uint8_t *smem)
+__device__ __forceinline__ void run(const SampleParams &P, uint8_t *smem, int cta)
 {
     const SmemLayout &L = P.L;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n = P.n_streams;
-    const int cta_s0 = blockIdx.x * S;
+    const int cta_s0 = cta * S;
     const int spf = P.spf;
 
     const uint32_t bar = smem_u32(smem + FN_MBAR);
@@ -315,7 +317,20 @@ template <int S>
 __global__ void __launch_bounds__(FN_THREADS, 1) lpcnet_sample_kernel_f32n(const __grid_constant__ SampleParams P)
 {
     extern __shared__ __align__(128) uint8_t smem[];
-    run<S>(P, smem);
+    run<S>(P, smem, blockIdx.x);
+}
+
+// Several float batches of one GRU_A size in one launch: member k holds CTAs [cta0[k], cta0[k+1]) (GroupSampleParams, engine.h),
+// S streams each.  Every m[k] carries the member's neuron-per-lane layout and image (DeviceModel::Ln / image_n).
+template <int S>
+__global__ void __launch_bounds__(FN_THREADS, 1) lpcnet_group_sample_kernel_f32n(const __grid_constant__ GroupSampleParams G)
+{
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int c = blockIdx.x;
+    int k = 0;
+#pragma unroll 1
+    for (int j = 1; j < G.count; j++) if (c >= G.cta0[j]) k = j;
+    run<S>(G.m[k], smem, c - G.cta0[k]);
 }
 
 cudaError_t launch_sample_kernel_f32n(const SampleParams &p, cudaStream_t st)
@@ -326,6 +341,17 @@ cudaError_t launch_sample_kernel_f32n(const SampleParams &p, cudaStream_t st)
     if (e != cudaSuccess) return e;
     const int ctas = (p.n_streams + S - 1) / S;
     kern<<<ctas, FN_THREADS, p.L.total_bytes, st>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_group_sample_kernel_f32n(const GroupSampleParams &g, int ctas, uint32_t smem_bytes, cudaStream_t st)
+{
+    const int spc = g.m[0].spc;                                   // (the same in every member: the group's plan)
+    void (*kern)(GroupSampleParams) = spc <= 1 ? lpcnet_group_sample_kernel_f32n<1> : spc == 2 ? lpcnet_group_sample_kernel_f32n<2>
+                                                                                               : lpcnet_group_sample_kernel_f32n<FN_S>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    kern<<<ctas, FN_THREADS, smem_bytes, st>>>(g);
     return cudaGetLastError();
 }
 

@@ -6,7 +6,11 @@ separates the launch plan from the L2 footprint of K models' embedding tables.  
 member) and 1024 streams per member.  Every step synthesizes 10 frames (160 samples each) per stream; timed with CUDA events
 on one caller stream after warm-up.  Prints one JSON line per case plus the card's name and power limit.
 
-    python tools/bench_group.py [--steps 10] [--warmup 3] [--ks 1,2,4,8]"""
+--flavour float measures float models instead (gen_model.make_model(seed) float blobs, seeded members only) at 32, 64, 128 and
+1024 streams per member: these sizes reach both float kernels (neuron-per-lane at up to 4 streams per CTA, lane == stream above)
+and the batches that leave SMs idle on their own.
+
+    python tools/bench_group.py [--steps 10] [--warmup 3] [--ks 1,2,4,8] [--flavour int8|float]"""
 import argparse
 import json
 import os
@@ -32,11 +36,11 @@ def card():
     return out
 
 
-def blob_for(seed):
+def blob_for(seed, flavour="int8"):
     import gen_model
     import lpcnet_b200
-    common, only8, _ = gen_model.make_model(seed)
-    return lpcnet_b200.write_blob([(n, t, a.tobytes()) for n, t, a in common + only8])
+    common, only8, onlyf = gen_model.make_model(seed)
+    return lpcnet_b200.write_blob([(n, t, a.tobytes()) for n, t, a in common + (onlyf if flavour == "float" else only8)])
 
 
 def features(n, torch):
@@ -102,6 +106,7 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--ks", default="1,2,4,8")
+    ap.add_argument("--flavour", choices=["int8", "float"], default="int8")
     a = ap.parse_args()
     import torch
     import lpcnet_b200
@@ -109,7 +114,15 @@ def main():
     build.build()
     print(json.dumps(dict(card=card())), flush=True)
     ks = [int(k) for k in a.ks.split(",")]
-    seeded = [blob_for(1234 + 17 * i) for i in range(max(ks))]
+    seeded = [blob_for(1234 + 17 * i, a.flavour) for i in range(max(ks))]
+    if a.flavour == "float":
+        for per_member in (32, 64, 128, 1024):
+            for K in ks:
+                r = run_case(lpcnet_b200, torch, seeded[:K], per_member, a.steps, a.warmup)
+                r.update(models="seeds", flavour="float")
+                print(json.dumps(r), flush=True)
+        print(json.dumps(dict(card=card())), flush=True)
+        return
     for models in ("seeds", "same"):
         for K in ks:
             if models == "same" and K == 1:
