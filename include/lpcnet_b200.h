@@ -241,7 +241,8 @@ LPCNET_EXPORT int lpcnet_b200_batch_decode_device(LPCNetB200Batch *b, const unsi
  * The per-stream lifecycle calls (reset, tail, deferred / flush, export / import, snapshots, codebooks) stay on the members,
  * which keep their own switches (FEATURES_DELAY, END2END, LPC_GAMMA) and sparsity patterns.  Group calls are ordered with
  * the members' own calls like any other call, so `_device` group calls may be mixed with member calls on any stream.
- * A member with a PCM sink set is refused.  The group does not own its members: destroy the group before any member.
+ * A member with a PCM sink set is refused (multi-GPU groups below gather the PCM themselves).  The group does not own its members:
+ * destroy the group before any member.
  * Float groups pick their kernel as a float batch does: the neuron-per-lane kernel while the plan's streams per CTA is at most
  * 4, the lane == stream kernel above that (or always, with LPCNET_B200_FLOAT_LANE_STREAM set at create).
  * group_create returns NULL (message: lpcnet_b200_last_error) for members on different devices, with different GRU_A
@@ -274,6 +275,43 @@ LPCNET_EXPORT int lpcnet_b200_debug_group_plan(const int *n, int count, int sms,
  * kernel, -1 for bad arguments. */
 LPCNET_EXPORT int lpcnet_b200_debug_group_plan_float(const int *n, int count, int sms, int override_spc, int lane_stream,
                                                      int *spc, int *slots, int *ctas);
+
+/* == multi-GPU groups: several models over every GPU of the process in one call ==
+ * The members are existing multi-GPU objects (lpcnet_b200_multi_create), one per model, all over the same device list in the same
+ * order, with one GRU_A size and one flavour (all int8 or all float), each at most once (at most 16).  Each keeps its own stream
+ * count and sharding; shard k of every member sits on devices[k].  For each device the multi-group holds one group
+ * (lpcnet_b200_group_create) over that device's shard batches, in member order, so every device runs each member's frame
+ * network and silent-frame launches, then one per-sample launch per chunk for all of them.  Every call enqueues all devices, each
+ * on a stream of its own, then waits for all of them.
+ * Job row r = member 0's streams in its own order, then member 1's, ... (the sum of their sizes, lpcnet_b200_multi_group_streams);
+ * features, packets and PCM are laid out as for lpcnet_b200_multi_* with that many streams.  `_gather` calls collect the PCM in the
+ * memory of devices[0] ([sum n][T] int16): every finished chunk (<= 16 frames) of every member's shard travels to its rows there
+ * on a copy stream (peer DMA when lpcnet_b200_multi_peer_access allows it, staged by the driver otherwise) while the next chunk is
+ * computed; the call returns once the gathered PCM is complete.  As for lpcnet_b200_multi_*, pinned host buffers
+ * (lpcnet_b200_host_alloc) let the copies of different devices overlap.
+ * A call leaves every member exactly as the member's own lpcnet_b200_multi_synthesize / _decode on its rows of the inputs would:
+ * PCM, recurrent state, RNG, frame counters, decoder memory, what a later tail reads.  Multi-group calls are ordered with every
+ * other call on the shard batches, so they may be mixed with member multi calls, shard lifecycle calls (reset_streams,
+ * export / import, copy_streams) and single-device group calls over the shards.  A PCM sink a member's own `_gather` call left on a
+ * shard batch is neither used nor cleared.  Bad arguments (feature_stride < 20, samples_per_frame outside 1..65536, a decode
+ * with a member that has no codebooks) are refused before anything is enqueued on any device.
+ * create returns NULL (message: lpcnet_b200_last_error) and changes nothing for a NULL argument, count outside 1..16, a member
+ * listed twice, members over different device lists, different GRU_A sizes, or int8 and float members mixed.  The multi-group
+ * does not own its members: destroy it before any of them. */
+typedef struct LPCNetB200MultiGroup LPCNetB200MultiGroup;
+LPCNET_EXPORT LPCNetB200MultiGroup *lpcnet_b200_multi_group_create(LPCNetB200Multi *const *members, int count);
+LPCNET_EXPORT void lpcnet_b200_multi_group_destroy(LPCNetB200MultiGroup *mg);
+LPCNET_EXPORT int lpcnet_b200_multi_group_streams(const LPCNetB200MultiGroup *mg);
+/* the group of devices[k] (lpcnet_b200_group_last_sample_kernel_ms of that device's last call, introspection) */
+LPCNET_EXPORT LPCNetB200Group *lpcnet_b200_multi_group_group(LPCNetB200MultiGroup *mg, int k);
+/* features [sum n][nframes][feature_stride] -> pcm [sum n][nframes*samples_per_frame] on the host / gathered on devices[0] */
+LPCNET_EXPORT int lpcnet_b200_multi_group_synthesize(LPCNetB200MultiGroup *mg, const float *features, int nframes, int feature_stride,
+                                                     int samples_per_frame, short *pcm);
+LPCNET_EXPORT int lpcnet_b200_multi_group_synthesize_gather(LPCNetB200MultiGroup *mg, const float *features, int nframes,
+                                                            int feature_stride, int samples_per_frame, short *d_pcm);
+/* packets [sum n][npackets][8] -> pcm [sum n][npackets*640]; every member needs its codebooks */
+LPCNET_EXPORT int lpcnet_b200_multi_group_decode(LPCNetB200MultiGroup *mg, const unsigned char *packets, int npackets, short *pcm);
+LPCNET_EXPORT int lpcnet_b200_multi_group_decode_gather(LPCNetB200MultiGroup *mg, const unsigned char *packets, int npackets, short *d_pcm);
 
 /* == the analysis side, batched (SURVEY 8f N2): feature extraction and the 1.6 kb/s encoder ==
  * n independent LPCNetEncState streams (reference src/lpcnet_private.h:55-75) on one device, all starting from

@@ -126,6 +126,16 @@ def lib():
     L.lpcnet_b200_shard_range.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p]
     L.lpcnet_b200_device_alloc_on.restype = c_p
     L.lpcnet_b200_device_alloc_on.argtypes = [ctypes.c_int, ctypes.c_size_t]
+    L.lpcnet_b200_multi_group_create.restype = c_p
+    L.lpcnet_b200_multi_group_create.argtypes = [c_p, ctypes.c_int]
+    L.lpcnet_b200_multi_group_destroy.argtypes = [c_p]
+    L.lpcnet_b200_multi_group_streams.argtypes = [c_p]
+    L.lpcnet_b200_multi_group_group.restype = c_p
+    L.lpcnet_b200_multi_group_group.argtypes = [c_p, ctypes.c_int]
+    L.lpcnet_b200_multi_group_synthesize.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p]
+    L.lpcnet_b200_multi_group_synthesize_gather.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p]
+    L.lpcnet_b200_multi_group_decode.argtypes = [c_p, c_p, ctypes.c_int, c_p]
+    L.lpcnet_b200_multi_group_decode_gather.argtypes = [c_p, c_p, ctypes.c_int, c_p]
     # analysis side (csrc/enc_kernels.cu)
     L.lpcnet_b200_enc_create.restype = c_p
     L.lpcnet_b200_enc_create.argtypes = [ctypes.c_int, ctypes.c_int]
@@ -700,6 +710,97 @@ class Group:
         k = ctypes.c_int(0)
         ms = self._L.lpcnet_b200_group_last_sample_kernel_ms(self._h, ctypes.byref(k))
         return float(ms), int(k.value)
+
+
+class _OwnedGroup(Group):
+    """a group another object holds (MultiGroup.group): the same calls, but closing it leaves the group alone"""
+
+    def __init__(self, h, owner):
+        self._L = lib()
+        self._h, self._owner, self.batches = h, owner, None
+        self.n = int(self._L.lpcnet_b200_group_streams(h))
+
+    def close(self):
+        self._h = None
+
+    __del__ = close
+
+
+class MultiGroup:
+    """Several Multi objects, one per model, all over the same devices and of one flavour and GRU_A size, served by one call: on
+    every device one group over the members' shards (lpcnet_b200_multi_group_*).  Rows = multis[0]'s streams, then multis[1]'s, ...
+    The members stay usable on their own; the multi-group keeps them alive and must be closed before they are."""
+
+    def __init__(self, multis):
+        self._L = lib()
+        self.multis = list(multis)
+        hs = (c_p * len(self.multis))(*[m._h for m in self.multis])
+        self._h = self._L.lpcnet_b200_multi_group_create(hs, len(self.multis))
+        if not self._h:
+            raise LPCNetB200Error("lpcnet_b200_multi_group_create: " + _err())
+        self.n = int(self._L.lpcnet_b200_multi_group_streams(self._h))
+        self.devices = list(self.multis[0].devices)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.lpcnet_b200_multi_group_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def group(self, k):
+        """the group of devices[k] (last_sample_kernel_ms of its part of the last call)"""
+        h = self._L.lpcnet_b200_multi_group_group(self._h, int(k))
+        if not h:
+            raise LPCNetB200Error(_err())
+        return _OwnedGroup(h, self)
+
+    def _gathered(self, call, pcm):
+        d = self._L.lpcnet_b200_device_alloc_on(self.devices[0], pcm.nbytes)
+        if not d:
+            raise LPCNetB200Error(_err())
+        try:
+            call(d)
+            self._L.lpcnet_b200_set_device(self.devices[0])
+            if self._L.lpcnet_b200_memcpy_d2h(pcm.ctypes.data, d, pcm.nbytes) != 0:
+                raise LPCNetB200Error(_err())
+        finally:
+            self._L.lpcnet_b200_device_free(d)
+        return pcm
+
+    def synthesize(self, features, samples_per_frame=160, gather=False):
+        """features [sum n][T][stride>=20] -> pcm [sum n][T*spf]; gather=True collects the PCM on devices[0] first and reads it back
+        from there."""
+        f = np.ascontiguousarray(features, dtype=np.float32)
+        if f.ndim != 3 or f.shape[0] != self.n:
+            raise LPCNetB200Error("multi_group synthesize: features of shape %s for %d streams" % (f.shape, self.n))
+        T, stride = f.shape[1], f.shape[2]
+        pcm = np.zeros((self.n, T * samples_per_frame), dtype=np.int16)
+
+        def call(d):
+            fn = self._L.lpcnet_b200_multi_group_synthesize_gather if d else self._L.lpcnet_b200_multi_group_synthesize
+            if fn(self._h, f.ctypes.data, T, stride, samples_per_frame, d or pcm.ctypes.data) != 0:
+                raise LPCNetB200Error("lpcnet_b200_multi_group_synthesize%s: %s" % ("_gather" if d else "", _err()))
+        if gather:
+            return self._gathered(call, pcm)
+        call(None)
+        return pcm
+
+    def decode(self, packets, gather=False):
+        """packets [sum n][P][8] uint8 -> pcm [sum n][P*640] int16."""
+        p = np.ascontiguousarray(packets, dtype=np.uint8)
+        if p.ndim != 3 or p.shape[0] != self.n or p.shape[2] != 8:
+            raise LPCNetB200Error("multi_group decode: packets of shape %s for %d streams" % (p.shape, self.n))
+        pcm = np.zeros((self.n, p.shape[1] * 640), dtype=np.int16)
+
+        def call(d):
+            fn = self._L.lpcnet_b200_multi_group_decode_gather if d else self._L.lpcnet_b200_multi_group_decode
+            if fn(self._h, p.ctypes.data, p.shape[1], d or pcm.ctypes.data) != 0:
+                raise LPCNetB200Error("lpcnet_b200_multi_group_decode%s: %s" % ("_gather" if d else "", _err()))
+        if gather:
+            return self._gathered(call, pcm)
+        call(None)
+        return pcm
 
 
 class LPCNet:

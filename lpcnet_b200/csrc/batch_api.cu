@@ -560,19 +560,26 @@ static int sample_frames(LPCNetB200Batch *b, int pos0, int nf, int spf, short *p
     return launches;
 }
 
-// chunk [c0, c0+nf) of a call is complete on `st`: forward its PCM block to the sink (if one is set) on the copy stream
+// chunk [c0, c0+nf) of the n PCM rows at d_pcm is complete on `st`: forward its block to target t on the copy stream `cs`, which
+// overlaps the next chunk's kernels (`ev`: the copy stream's hand-over event)
+static int forward_chunk(const PcmTarget &t, int n, const short *d_pcm, long long pcm_stride, int c0, int nf, int spf, cudaStream_t st,
+                         cudaStream_t cs, cudaEvent_t ev)
+{
+    CK(cudaEventRecord(ev, st));
+    CK(cudaStreamWaitEvent(cs, ev, 0));
+    short *dst = t.dst + t.row0 * t.pitch + (size_t)c0 * spf;
+    if (c0 == 0 && (long long)nf * spf == pcm_stride && t.pitch == pcm_stride)      // whole rows, same pitch: one contiguous block (one DMA descriptor
+        CK(cudaMemcpyAsync(dst, d_pcm, (size_t)n * pcm_stride * sizeof(short), cudaMemcpyDefault, cs));   // instead of n row copies)
+    else
+        CK(cudaMemcpy2DAsync(dst, t.pitch * sizeof(short), d_pcm + (size_t)c0 * spf, pcm_stride * sizeof(short), (size_t)nf * spf * sizeof(short), n,
+                             cudaMemcpyDefault, cs));       // (the target may live on another device: UVA infers the route)
+    return 0;
+}
+// ... to the batch's sink, if one is set
 static int forward_to_sink(LPCNetB200Batch *b, const short *d_pcm, long long pcm_stride, int c0, int nf, int spf, cudaStream_t st)
 {
     if (!b->sink) return 0;
-    CK(cudaEventRecord(b->sink_ev, st));
-    CK(cudaStreamWaitEvent(b->sink_stream, b->sink_ev, 0));
-    short *dst = b->sink + b->sink_row0 * b->sink_pitch + (size_t)c0 * spf;
-    if (c0 == 0 && (long long)nf * spf == pcm_stride && b->sink_pitch == pcm_stride)      // whole rows, same pitch: one contiguous block (one DMA descriptor
-        CK(cudaMemcpyAsync(dst, d_pcm, (size_t)b->n * pcm_stride * sizeof(short), cudaMemcpyDefault, b->sink_stream));   // instead of n row copies)
-    else
-        CK(cudaMemcpy2DAsync(dst, b->sink_pitch * sizeof(short), d_pcm + (size_t)c0 * spf, pcm_stride * sizeof(short), (size_t)nf * spf * sizeof(short), b->n,
-                             cudaMemcpyDefault, b->sink_stream));       // (the sink may live on another device: UVA infers the route)
-    return 0;
+    return forward_chunk(PcmTarget{b->sink, b->sink_pitch, b->sink_row0}, b->n, d_pcm, pcm_stride, c0, nf, spf, st, b->sink_stream, b->sink_ev);
 }
 
 // The 100 Hz part of a chunk [c0, c0 + nf) of a call: the frame network on the batch's rows of the features; the chunk's last
@@ -843,6 +850,7 @@ struct LPCNetB200Group {
     cudaStream_t stream;
     std::vector<cudaEvent_t> kev;     // event pairs around the group's own per-sample launches of the last call
     int kev_used, last_launches;
+    cudaStream_t fwd_stream; cudaEvent_t fwd_ev, fwd_done;   // copy stream of the forwarded PCM (group_*_forward), made on first use
 };
 
 // One streams-per-CTA value for the whole launch: the smallest that puts every member on at most `sms` CTAs in total, member k
@@ -890,6 +898,9 @@ void lpcnet_b200_group_destroy(LPCNetB200Group *g)
     if (!g) return;
     cudaSetDevice(g->device);
     if (g->stream) { cudaStreamSynchronize(g->stream); cudaStreamDestroy(g->stream); }
+    if (g->fwd_stream) { cudaStreamSynchronize(g->fwd_stream); cudaStreamDestroy(g->fwd_stream); }
+    if (g->fwd_ev) cudaEventDestroy(g->fwd_ev);
+    if (g->fwd_done) cudaEventDestroy(g->fwd_done);
     for (cudaEvent_t e : g->kev) cudaEventDestroy(e);
     delete g;
 }
@@ -974,13 +985,21 @@ static int launch_group(LPCNetB200Group *g, const int *live0, int nf, int spf, s
 }
 
 // Core of the group calls: member k reads features feat[k] ([n_k][nframes][frame_stride]) and writes pcm[k] ([n_k][nframes*spf]),
-// all device pointers, everything on `st`.  Per chunk: every member's frame network, every member's silent prefix, one launch.
-static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_stride, int nframes, int spf, short *const *pcm, cudaStream_t st)
+// all device pointers, everything on `st`.  Per chunk: every member's frame network, every member's silent prefix, one launch, and
+// the chunk's PCM forwarded to fwd[k] for the members that have a target (fwd NULL: none).
+static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_stride, int nframes, int spf, short *const *pcm,
+                       const PcmTarget *fwd, cudaStream_t st)
 {
     if (nframes <= 0) return 0;
-    if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
-    if (frame_stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
+    if (group_call_check(g, nframes, frame_stride, spf, false)) return -1;
     const long long stream_stride = (long long)nframes * frame_stride, pcm_stride = (long long)nframes * spf;
+    bool forwarding = false;
+    for (int k = 0; fwd && k < g->count; k++) forwarding = forwarding || fwd[k].dst;
+    if (forwarding && !g->fwd_stream) {
+        CK(cudaStreamCreateWithFlags(&g->fwd_stream, cudaStreamNonBlocking));
+        CK(cudaEventCreateWithFlags(&g->fwd_ev, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&g->fwd_done, cudaEventDisableTiming));
+    }
     int launches = 0;
     g->kev_used = 0;
     for (int k = 0; k < g->count; k++) {
@@ -1003,8 +1022,14 @@ static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_s
         if (r < 0) return -1;
         launches += r;
         for (int k = 0; k < g->count; k++) for (int &v : g->m[k]->fc) v = std::min(1000, v + nf);
+        for (int k = 0; forwarding && k < g->count; k++)
+            if (fwd[k].dst && forward_chunk(fwd[k], g->m[k]->n, pcm[k], pcm_stride, c0, nf, spf, st, g->fwd_stream, g->fwd_ev)) return -1;
     }
     CK(cudaGetLastError());
+    if (forwarding) {    // the call's completion includes the forwarded PCM
+        CK(cudaEventRecord(g->fwd_done, g->fwd_stream));
+        CK(cudaStreamWaitEvent(st, g->fwd_done, 0));
+    }
     for (int k = 0; k < g->count; k++) if (order_leave(g->m[k], st)) return -1;
     g->last_launches = launches;
     return 0;
@@ -1026,14 +1051,7 @@ int lpcnet_b200_group_synthesize_device(LPCNetB200Group *g, const float *d_featu
     if (nframes <= 0) return 0;
     if (!d_features || !d_pcm) { set_error("null buffer"); return -1; }
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
-    const float *feat[GROUP_MAX]; short *pcm[GROUP_MAX];
-    size_t row = 0;
-    for (int k = 0; k < g->count; k++) {
-        feat[k] = d_features + row * nframes * feature_stride;
-        pcm[k] = d_pcm + row * nframes * samples_per_frame;
-        row += g->m[k]->n;
-    }
-    int r = group_synth(g, feat, feature_stride, nframes, samples_per_frame, pcm, st);
+    int r = group_synthesize_forward(g, d_features, nframes, feature_stride, samples_per_frame, d_pcm, nullptr, st);
     if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
     return r;
 }
@@ -1060,7 +1078,7 @@ int lpcnet_b200_group_synthesize(LPCNetB200Group *g, const float *features, int 
         if (order_leave(b, g->stream)) return -1;
         row += b->n;
     }
-    if (group_synth(g, feat, feature_stride, nframes, samples_per_frame, dp, g->stream)) return -1;
+    if (group_synth(g, feat, feature_stride, nframes, samples_per_frame, dp, nullptr, g->stream)) return -1;
     row = 0;
     for (int k = 0; k < g->count; k++) {
         LPCNetB200Batch *b = g->m[k];
@@ -1073,12 +1091,12 @@ int lpcnet_b200_group_synthesize(LPCNetB200Group *g, const float *features, int 
 }
 
 // decode: every member's packet decoder into the member's feature staging, then the group synthesis over those features
-static int group_decode(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, cudaStream_t st)
+static int group_decode(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, const PcmTarget *fwd, cudaStream_t st)
 {
+    if (group_call_check(g, npackets * 4, NB_FEAT, FRAME_SIZE, true)) return -1;
     const float *feat[GROUP_MAX];
     for (int k = 0; k < g->count; k++) {
         LPCNetB200Batch *b = g->m[k];
-        if (!b->model.codebooks) { set_error("group decode: member %d has no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)", k); return -1; }
         if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * (size_t)b->n * npackets * 4 * NB_FEAT)) return -1;
         feat[k] = b->d_features;
     }
@@ -1088,10 +1106,53 @@ static int group_decode(LPCNetB200Group *g, const uint8_t *const *packets, int n
         launch_decode_packets(b->model, b->fs, packets[k], b->n, npackets, b->d_features, st);
         if (order_leave(b, st)) return -1;
     }
-    if (group_synth(g, feat, NB_FEAT, npackets * 4, FRAME_SIZE, pcm, st)) return -1;
+    if (group_synth(g, feat, NB_FEAT, npackets * 4, FRAME_SIZE, pcm, fwd, st)) return -1;
     g->last_launches += g->count;
     return 0;
 }
+
+}  // extern "C"
+
+// ---- the entries of the multi-GPU groups (engine.h) ----
+int lpcnet_b200::group_call_check(const LPCNetB200Group *g, int nframes, int frame_stride, int spf, bool decode)
+{
+    if (!g) { set_error("null group"); return -1; }
+    if (nframes <= 0) return 0;
+    if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
+    if (frame_stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
+    if (decode)
+        for (int k = 0; k < g->count; k++)
+            if (!g->m[k]->model.codebooks) { set_error("group decode: member %d has no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)", k); return -1; }
+    return 0;
+}
+
+// group rows in one device buffer each: member k's features and PCM at its first row
+int lpcnet_b200::group_synthesize_forward(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride, int spf, short *d_pcm,
+                                          const PcmTarget *fwd, cudaStream_t st)
+{
+    const float *feat[GROUP_MAX] = {}; short *pcm[GROUP_MAX] = {};
+    size_t row = 0;
+    for (int k = 0; k < g->count; k++) {
+        feat[k] = d_features + row * nframes * feature_stride;
+        pcm[k] = d_pcm + row * nframes * spf;
+        row += g->m[k]->n;
+    }
+    return group_synth(g, feat, feature_stride, nframes, spf, pcm, fwd, st);
+}
+
+int lpcnet_b200::group_decode_forward(LPCNetB200Group *g, const uint8_t *d_packets, int npackets, short *d_pcm, const PcmTarget *fwd, cudaStream_t st)
+{
+    const uint8_t *pk[GROUP_MAX] = {}; short *pcm[GROUP_MAX] = {};
+    size_t row = 0;
+    for (int k = 0; k < g->count; k++) {
+        pk[k] = d_packets + row * npackets * 8;
+        pcm[k] = d_pcm + row * npackets * 640;
+        row += g->m[k]->n;
+    }
+    return group_decode(g, pk, npackets, pcm, fwd, st);
+}
+
+extern "C" {
 
 int lpcnet_b200_group_decode_device(LPCNetB200Group *g, const unsigned char *d_packets, int npackets, short *d_pcm, void *cuda_stream)
 {
@@ -1099,14 +1160,7 @@ int lpcnet_b200_group_decode_device(LPCNetB200Group *g, const unsigned char *d_p
     if (npackets <= 0) return 0;
     if (!d_packets || !d_pcm) { set_error("null buffer"); return -1; }
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
-    const uint8_t *pk[GROUP_MAX]; short *pcm[GROUP_MAX];
-    size_t row = 0;
-    for (int k = 0; k < g->count; k++) {
-        pk[k] = d_packets + row * npackets * 8;
-        pcm[k] = d_pcm + row * npackets * 640;
-        row += g->m[k]->n;
-    }
-    int r = group_decode(g, pk, npackets, pcm, st);
+    int r = group_decode_forward(g, d_packets, npackets, d_pcm, nullptr, st);
     if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
     return r;
 }
@@ -1131,7 +1185,7 @@ int lpcnet_b200_group_decode(LPCNetB200Group *g, const unsigned char *packets, i
         if (order_leave(b, g->stream)) return -1;
         row += b->n;
     }
-    if (group_decode(g, pk, npackets, dp, g->stream)) return -1;
+    if (group_decode(g, pk, npackets, dp, nullptr, g->stream)) return -1;
     row = 0;
     for (int k = 0; k < g->count; k++) {
         LPCNetB200Batch *b = g->m[k];

@@ -405,3 +405,19 @@ int sample_kernel_smem_ok(uint32_t bytes);
 int streams_per_cta_for(int n_streams, int override_spc);   // min(32, ceil(n / SM count)) on the current device unless overridden
 
 }  // namespace lpcnet_b200
+
+// ---- group calls with per-member PCM forwarding (batch_api.cu; used by the multi-GPU groups of multi_api.cu) ----
+struct LPCNetB200Group;
+namespace lpcnet_b200 {
+// Where a member's PCM goes as well: after every chunk, rows s of the member's PCM land at dst[(row0 + s) * pitch + t] (dst NULL: nowhere)
+struct PcmTarget { short *dst; long long pitch, row0; };
+// Refuses (sets the error, returns -1) what a group synthesize call of nframes frames would refuse (decode: a decode call of
+// nframes / 4 packets, frame_stride 20, spf 160), without enqueueing anything.
+int group_call_check(const LPCNetB200Group *g, int nframes, int frame_stride, int spf, bool decode);
+// The group's synthesize / decode `_device` calls with fwd[k] as member k's target (fwd NULL: none).  Members' PCM sinks are
+// neither used nor refused.  Everything is enqueued on `st` (of the group's device, current); the forwarded copies are part of
+// the call's completion on `st`.
+int group_synthesize_forward(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride, int spf, short *d_pcm,
+                             const PcmTarget *fwd, cudaStream_t st);
+int group_decode_forward(LPCNetB200Group *g, const uint8_t *d_packets, int npackets, short *d_pcm, const PcmTarget *fwd, cudaStream_t st);
+}  // namespace lpcnet_b200

@@ -10,6 +10,9 @@
 //     pushed by that device's copy engine over NVLink into the gather buffer (peer access) while the next chunk is being
 //     computed (LPCNetB200Batch's PCM sink, batch_api.cu forward_to_sink).
 // One process per GPU (torchrun / MPI style) uses the same sink through CUDA IPC instead: lpcnet_b200_ipc_export/_open.
+// Multi-GPU groups (lpcnet_b200_multi_group_*) serve several models, one LPCNetB200Multi each over the same devices, the same way:
+// per device one group over the members' shards, and the gather forwarded from inside the group's chunk loop
+// (batch_api.cu group_synthesize_forward) instead of through the shard batches' sinks.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -193,6 +196,170 @@ int lpcnet_b200_multi_decode_gather(LPCNetB200Multi *m, const unsigned char *pac
     if (!m || !packets || !d_pcm) { set_error("multi_decode_gather: null argument"); return -1; }
     if (npackets <= 0) return 0;
     return run_all(m, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, nullptr, d_pcm);
+}
+
+// ---- multi-GPU groups: several models, each an LPCNetB200Multi over the same devices, in one call ----
+// Device k runs one LPCNetB200Group over shard k of every member.  Job rows are member 0's streams, then member 1's, ...; on device k
+// the rows of member m are base[m] + first_mk .. + count_mk, staged in the device's buffers as one block per member, in member order
+// (the group's own row layout).
+struct MGDevice {
+    int device, rows;                     // rows: sum over the members of their shard's streams on this device
+    LPCNetB200Group *group;
+    cudaStream_t stream;
+    void *d_in; size_t d_in_cap;
+    short *d_pcm; size_t d_pcm_cap;
+};
+
+struct LPCNetB200MultiGroup {
+    int n;
+    std::vector<LPCNetB200Multi *> m;
+    std::vector<int> base;                // first job row of each member
+    std::vector<MGDevice> dev;
+};
+
+void lpcnet_b200_multi_group_destroy(LPCNetB200MultiGroup *mg)
+{
+    if (!mg) return;
+    for (MGDevice &d : mg->dev) {
+        cudaSetDevice(d.device);
+        if (d.stream) cudaStreamSynchronize(d.stream);
+        if (d.group) lpcnet_b200_group_destroy(d.group);
+        if (d.d_in) cudaFree(d.d_in);
+        if (d.d_pcm) cudaFree(d.d_pcm);
+        if (d.stream) cudaStreamDestroy(d.stream);
+    }
+    delete mg;
+}
+
+LPCNetB200MultiGroup *lpcnet_b200_multi_group_create(LPCNetB200Multi *const *members, int count)
+{
+    if (!members || count < 1 || count > GROUP_MAX) { set_error("multi_group_create: 1..%d member multis", GROUP_MAX); return nullptr; }
+    int na0 = 0;
+    for (int k = 0; k < count; k++) {
+        const LPCNetB200Multi *m = members[k];
+        if (!m) { set_error("multi_group_create: member %d is NULL", k); return nullptr; }
+        for (int j = 0; j < k; j++) if (members[j] == m) { set_error("multi_group_create: member %d is listed twice (also member %d)", k, j); return nullptr; }
+        const std::vector<Shard> &s = m->shards, &s0 = members[0]->shards;
+        bool same = s.size() == s0.size();
+        for (size_t i = 0; same && i < s.size(); i++) same = s[i].device == s0[i].device;
+        if (!same) { set_error("multi_group_create: member %d runs on other devices than member 0 (the device lists must be equal, in order)", k); return nullptr; }
+        int na = 0;
+        lpcnet_b200_batch_model_info(s[0].batch, &na, nullptr);
+        if (k == 0) na0 = na;
+        if (na != na0) { set_error("multi_group_create: member %d has %d GRU_A units, member 0 has %d", k, na, na0); return nullptr; }
+        const int fl = lpcnet_b200_batch_is_float(s[0].batch), fl0 = lpcnet_b200_batch_is_float(s0[0].batch);
+        if (fl != fl0) {
+            set_error("multi_group_create: member %d holds %s model, member 0 %s one; the members are all int8 or all float", k,
+                      fl ? "a float" : "an int8", fl0 ? "a float" : "an int8");
+            return nullptr;
+        }
+    }
+    LPCNetB200MultiGroup *mg = new LPCNetB200MultiGroup();
+    mg->m.assign(members, members + count);
+    for (LPCNetB200Multi *m : mg->m) { mg->base.push_back(mg->n); mg->n += m->n; }
+    const size_t nd = members[0]->shards.size();
+    for (size_t k = 0; k < nd; k++) {
+        MGDevice d; memset(&d, 0, sizeof(d));
+        d.device = members[0]->shards[k].device;
+        mg->dev.push_back(d);
+    }
+    for (size_t k = 0; k < nd; k++) {
+        MGDevice &d = mg->dev[k];
+        LPCNetB200Batch *b[GROUP_MAX];
+        for (int j = 0; j < count; j++) { b[j] = members[j]->shards[k].batch; d.rows += members[j]->shards[k].count; }
+        d.group = lpcnet_b200_group_create(b, count);          // (sets the current device)
+        if (!d.group || cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking) != cudaSuccess) {
+            if (d.group) set_error("multi_group_create: stream creation failed on device %d", d.device);
+            lpcnet_b200_multi_group_destroy(mg); return nullptr;
+        }
+    }
+    return mg;
+}
+
+int lpcnet_b200_multi_group_streams(const LPCNetB200MultiGroup *mg) { return mg ? mg->n : 0; }
+LPCNetB200Group *lpcnet_b200_multi_group_group(LPCNetB200MultiGroup *mg, int k)
+{
+    if (!mg || k < 0 || k >= (int)mg->dev.size()) { set_error("multi_group_group: bad device index"); return nullptr; }
+    return mg->dev[k].group;
+}
+
+// One device's share of a call, enqueued on its stream: every member's rows up, then the group call, which forwards each chunk to
+// the gather buffer if there is one
+static int mg_enqueue(LPCNetB200MultiGroup *mg, size_t k, const void *in, size_t in_row_bytes, int units, int stride, int spf, bool decode,
+                      long long T, short *d_gather)
+{
+    MGDevice &d = mg->dev[k];
+    CK(cudaSetDevice(d.device));
+    if (grow(&d.d_in, &d.d_in_cap, in_row_bytes * d.rows) || grow((void **)&d.d_pcm, &d.d_pcm_cap, sizeof(short) * (size_t)T * d.rows)) return -1;
+    PcmTarget fwd[GROUP_MAX];
+    int local = 0;
+    for (size_t j = 0; j < mg->m.size(); j++) {
+        const Shard &s = mg->m[j]->shards[k];
+        const long long row = mg->base[j] + s.first;
+        fwd[j] = PcmTarget{d_gather, T, row};
+        CK(cudaMemcpyAsync((char *)d.d_in + in_row_bytes * local, (const char *)in + in_row_bytes * row, in_row_bytes * s.count, cudaMemcpyHostToDevice, d.stream));
+        local += s.count;
+    }
+    return decode ? group_decode_forward(d.group, (const uint8_t *)d.d_in, units, d.d_pcm, d_gather ? fwd : nullptr, d.stream)
+                  : group_synthesize_forward(d.group, (const float *)d.d_in, units, stride, spf, d.d_pcm, d_gather ? fwd : nullptr, d.stream);
+}
+// ... and its rows of every member down to the host
+static int mg_download(LPCNetB200MultiGroup *mg, size_t k, long long T, short *pcm_host)
+{
+    MGDevice &d = mg->dev[k];
+    CK(cudaSetDevice(d.device));
+    int local = 0;
+    for (size_t j = 0; j < mg->m.size(); j++) {
+        const Shard &s = mg->m[j]->shards[k];
+        CK(cudaMemcpyAsync(pcm_host + (size_t)T * (mg->base[j] + s.first), d.d_pcm + (size_t)T * local, sizeof(short) * (size_t)T * s.count,
+                           cudaMemcpyDeviceToHost, d.stream));
+        local += s.count;
+    }
+    return 0;
+}
+
+static int mg_run(LPCNetB200MultiGroup *mg, const void *in, size_t in_row_bytes, int units, int stride, int spf, bool decode,
+                  short *pcm_host, short *d_gather)
+{
+    for (MGDevice &d : mg->dev)          // refuse before anything is enqueued on any device
+        if (group_call_check(d.group, decode ? units * 4 : units, decode ? NB_FEAT : stride, spf, decode)) return -1;
+    const long long T = decode ? (long long)units * 640 : (long long)units * spf;
+    int rc = 0;
+    // enqueue the work of every device first, the copies to the host after it (a copy to pageable memory returns only once it
+    // is done: it must not hold back the next device's work) ...
+    for (size_t k = 0; k < mg->dev.size() && rc == 0; k++) rc = mg_enqueue(mg, k, in, in_row_bytes, units, stride, spf, decode, T, d_gather);
+    for (size_t k = 0; pcm_host && k < mg->dev.size() && rc == 0; k++) rc = mg_download(mg, k, T, pcm_host);
+    // ... then wait for all of them (also on the error path: nothing may still be reading the caller's buffers)
+    for (MGDevice &d : mg->dev) {
+        cudaSetDevice(d.device);
+        if (cudaStreamSynchronize(d.stream) != cudaSuccess && rc == 0) { set_error("multi_group: device %d: %s", d.device, cudaGetErrorString(cudaGetLastError())); rc = -1; }
+    }
+    return rc;
+}
+
+int lpcnet_b200_multi_group_synthesize(LPCNetB200MultiGroup *mg, const float *features, int nframes, int feature_stride, int samples_per_frame, short *pcm)
+{
+    if (!mg || !features || !pcm) { set_error("multi_group_synthesize: null argument"); return -1; }
+    if (nframes <= 0) return 0;
+    return mg_run(mg, features, sizeof(float) * (size_t)nframes * feature_stride, nframes, feature_stride, samples_per_frame, false, pcm, nullptr);
+}
+int lpcnet_b200_multi_group_synthesize_gather(LPCNetB200MultiGroup *mg, const float *features, int nframes, int feature_stride, int samples_per_frame, short *d_pcm)
+{
+    if (!mg || !features || !d_pcm) { set_error("multi_group_synthesize_gather: null argument"); return -1; }
+    if (nframes <= 0) return 0;
+    return mg_run(mg, features, sizeof(float) * (size_t)nframes * feature_stride, nframes, feature_stride, samples_per_frame, false, nullptr, d_pcm);
+}
+int lpcnet_b200_multi_group_decode(LPCNetB200MultiGroup *mg, const unsigned char *packets, int npackets, short *pcm)
+{
+    if (!mg || !packets || !pcm) { set_error("multi_group_decode: null argument"); return -1; }
+    if (npackets <= 0) return 0;
+    return mg_run(mg, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, pcm, nullptr);
+}
+int lpcnet_b200_multi_group_decode_gather(LPCNetB200MultiGroup *mg, const unsigned char *packets, int npackets, short *d_pcm)
+{
+    if (!mg || !packets || !d_pcm) { set_error("multi_group_decode_gather: null argument"); return -1; }
+    if (npackets <= 0) return 0;
+    return mg_run(mg, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, nullptr, d_pcm);
 }
 
 // memory on a given device (the gather buffer lives on devices[0])
