@@ -276,6 +276,52 @@ LPCNET_EXPORT int lpcnet_b200_debug_group_plan(const int *n, int count, int sms,
 LPCNET_EXPORT int lpcnet_b200_debug_group_plan_float(const int *n, int count, int sms, int override_spc, int lane_stream,
                                                      int *spc, int *slots, int *ctas);
 
+/* == mixed groups: batches of different GRU_A sizes and flavours in one call ==
+ * 1..16 existing batches on ONE device, each at most once, of any GRU_A size (128, 256, 384) and either flavour.  Members are
+ * partitioned into classes by (GRU_A size, flavour), in order of first appearance, and each class is one ordinary group
+ * (lpcnet_b200_group_create's kernel, CTA layout and shared memory) over its members in member order.  All classes share one
+ * streams-per-CTA value: the one a group over ALL members would plan (lpcnet_b200_debug_group_plan: the smallest spc at which
+ * sum ceil(n_k / spc) <= SM count, 32 if none; LPCNET_B200_STREAMS_PER_CTA pins it), so that the classes' CTAs together fit on the
+ * SMs (a float class's CTAs lay out slots >= spc streams, see lpcnet_b200_debug_group_plan_float).  A one-shape member list plans
+ * exactly as its group.  LPCNET_B200_STREAMS_PER_CTA and LPCNET_B200_FLOAT_LANE_STREAM are read at create.
+ * A call checks every class as that class's group call would, and refuses before anything is enqueued on any stream.  It then
+ * runs class 0's group call on the call's stream and every other class's on a stream the mixed group owns, forked from the call's
+ * stream and joined back into it, so the classes' per-sample launches can run at the same time on disjoint SMs.  Whether they do
+ * is up to the hardware; results never depend on it.
+ * Mixed-group stream g = the streams of batches[0], then batches[1], ... in order; features, packets and PCM are laid out as for a
+ * batch of that many streams.  The contract is the group's: a call leaves every member in exactly the state its own call on its
+ * rows of the inputs would leave it in (PCM, recurrent state, RNG, frame counters, decoder memory, what a later tail reads), from
+ * any member state.  Calls are ordered with every other call on the members, so `_device` calls may be mixed with member calls,
+ * ordinary groups over the same batches and the members' lifecycle calls on any stream.  A member with a PCM sink is refused,
+ * as is a decode with a member that has no codebooks.
+ * create returns NULL (message: lpcnet_b200_last_error) for a NULL argument, count outside 1..16, a member listed twice or
+ * members on different devices.  The mixed group does not own its members: destroy it before any of them. */
+typedef struct LPCNetB200MixedGroup LPCNetB200MixedGroup;
+LPCNET_EXPORT LPCNetB200MixedGroup *lpcnet_b200_mixed_group_create(LPCNetB200Batch *const *batches, int count);
+LPCNET_EXPORT void lpcnet_b200_mixed_group_destroy(LPCNetB200MixedGroup *mg);
+LPCNET_EXPORT int lpcnet_b200_mixed_group_streams(const LPCNetB200MixedGroup *mg);
+LPCNET_EXPORT int lpcnet_b200_mixed_group_classes(const LPCNetB200MixedGroup *mg);
+/* class c's group (lpcnet_b200_group_last_sample_kernel_ms of its part of the last call, introspection); owned by the mixed group */
+LPCNET_EXPORT LPCNetB200Group *lpcnet_b200_mixed_group_group(LPCNetB200MixedGroup *mg, int c);
+/* features [sum n][nframes][feature_stride] -> pcm [sum n][nframes*samples_per_frame] */
+LPCNET_EXPORT int lpcnet_b200_mixed_group_synthesize(LPCNetB200MixedGroup *mg, const float *features, int nframes, int feature_stride,
+                                                     int samples_per_frame, short *pcm);
+LPCNET_EXPORT int lpcnet_b200_mixed_group_synthesize_device(LPCNetB200MixedGroup *mg, const float *d_features, int nframes,
+                                                            int feature_stride, int samples_per_frame, short *d_pcm, void *cuda_stream);
+/* packets [sum n][npackets][8] -> pcm [sum n][npackets*640]; every member needs its codebooks */
+LPCNET_EXPORT int lpcnet_b200_mixed_group_decode(LPCNetB200MixedGroup *mg, const unsigned char *packets, int npackets, short *pcm);
+LPCNET_EXPORT int lpcnet_b200_mixed_group_decode_device(LPCNetB200MixedGroup *mg, const unsigned char *d_packets, int npackets,
+                                                        short *d_pcm, void *cuda_stream);
+/* device time (ms) of the last call, from the fork on the call's stream to the join of every class (<0 on error, 0 before any call) */
+LPCNET_EXPORT float lpcnet_b200_mixed_group_last_call_ms(const LPCNetB200MixedGroup *mg);
+/* Test hook (host only, no CUDA): the plan of a mixed group whose member k has n[k] streams, na[k] GRU_A units and flavour is_float[k]
+ * (0 / 1) on `sms` SMs.  *spc as lpcnet_b200_debug_group_plan over all members; class_of[k] = member k's class; per class c:
+ * class_ctas[c] = its CTAs (int8: sum ceil(n_k / spc); float: sum ceil(n_k / slots), slots as lpcnet_b200_debug_group_plan_float) and
+ * class_neuron[c] = 1 for a float class on the neuron-per-lane kernel.  lane_stream != 0 stands for LPCNET_B200_FLOAT_LANE_STREAM.
+ * Returns the number of classes, -1 for bad arguments. */
+LPCNET_EXPORT int lpcnet_b200_debug_mixed_plan(const int *n, const int *na, const int *is_float, int count, int sms, int override_spc,
+                                               int lane_stream, int *spc, int *class_of, int *class_ctas, int *class_neuron);
+
 /* == multi-GPU groups: several models over every GPU of the process in one call ==
  * The members are existing multi-GPU objects (lpcnet_b200_multi_create), one per model, all over the same device list in the same
  * order, with one GRU_A size and one flavour (all int8 or all float), each at most once (at most 16).  Each keeps its own stream

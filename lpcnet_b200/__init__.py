@@ -6,5 +6,5 @@ This package only loads it through ctypes and mirrors the reference's operator i
 extension, so that tests and the benchmark read like calls into the reference library.  There is no Python
 compute path and no CPU fallback: without the built library or without a CUDA device every call raises.
 """
-from .api import (Batch, Group, group_plan, group_plan_float, Multi, MultiGroup, EncBatch, LPCNet, LPCNetDecoder, lib, LPCNetB200Error, device_count, measure_smem_peak,  # noqa: F401
+from .api import (Batch, Group, group_plan, group_plan_float, mixed_plan, MixedGroup, Multi, MultiGroup, EncBatch, LPCNet, LPCNetDecoder, lib, LPCNetB200Error, device_count, measure_smem_peak,  # noqa: F401
                   parse_blob, write_blob, blob_config, shard_range)

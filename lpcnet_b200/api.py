@@ -78,6 +78,21 @@ def lib():
     L.lpcnet_b200_group_last_sample_kernel_ms.argtypes = [c_p, c_p]
     L.lpcnet_b200_debug_group_plan.argtypes = [c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p]
     L.lpcnet_b200_debug_group_plan_float.argtypes = [c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
+    # mixed groups (several group shapes, one launch per shape on streams of their own)
+    L.lpcnet_b200_mixed_group_create.restype = c_p
+    L.lpcnet_b200_mixed_group_create.argtypes = [c_p, ctypes.c_int]
+    L.lpcnet_b200_mixed_group_destroy.argtypes = [c_p]
+    L.lpcnet_b200_mixed_group_streams.argtypes = [c_p]
+    L.lpcnet_b200_mixed_group_classes.argtypes = [c_p]
+    L.lpcnet_b200_mixed_group_group.restype = c_p
+    L.lpcnet_b200_mixed_group_group.argtypes = [c_p, ctypes.c_int]
+    L.lpcnet_b200_mixed_group_synthesize.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p]
+    L.lpcnet_b200_mixed_group_synthesize_device.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p]
+    L.lpcnet_b200_mixed_group_decode.argtypes = [c_p, c_p, ctypes.c_int, c_p]
+    L.lpcnet_b200_mixed_group_decode_device.argtypes = [c_p, c_p, ctypes.c_int, c_p, c_p]
+    L.lpcnet_b200_mixed_group_last_call_ms.restype = ctypes.c_float
+    L.lpcnet_b200_mixed_group_last_call_ms.argtypes = [c_p]
+    L.lpcnet_b200_debug_mixed_plan.argtypes = [c_p, c_p, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p, c_p]
     L.lpcnet_b200_batch_is_float.argtypes = [c_p]
     L.lpcnet_b200_batch_get_state.argtypes = [c_p, ctypes.c_int, c_p, c_p, c_p, c_p, c_p]
     L.lpcnet_b200_debug_frame_network.argtypes = [c_p, c_p, ctypes.c_int, ctypes.c_int, c_p, c_p, c_p]
@@ -657,6 +672,26 @@ def group_plan_float(sizes, sms, override_spc=0, lane_stream=False):
     return ("neuron" if r == 1 else "lane"), int(spc.value), int(slots.value), int(ctas.value)
 
 
+def mixed_plan(sizes, na, is_float, sms, override_spc=0, lane_stream=False):
+    """Launch plan of a mixed group whose member k has sizes[k] streams, na[k] GRU_A units and flavour is_float[k] on `sms` SMs:
+    (streams per CTA, class of each member, [(kernel, CTA count) per class]) with kernel "int8", "neuron" or "lane" (the float
+    kernels of group_plan_float); lane_stream stands for LPCNET_B200_FLOAT_LANE_STREAM (lpcnet_b200_debug_mixed_plan; host only,
+    needs no GPU)."""
+    k = len(sizes)
+    if len(na) != k or len(is_float) != k:
+        raise LPCNetB200Error("mixed_plan: sizes, na and is_float differ in length")
+    arr = lambda v: (ctypes.c_int * max(k, 1))(*[int(x) for x in v])
+    cls, ctas, neuron = arr([0] * k), arr([0] * k), arr([0] * k)
+    spc = ctypes.c_int(0)
+    r = lib().lpcnet_b200_debug_mixed_plan(arr(sizes), arr(na), arr(is_float), k, int(sms), int(override_spc), int(bool(lane_stream)),
+                                           ctypes.byref(spc), cls, ctas, neuron)
+    if r < 0:
+        raise LPCNetB200Error("debug_mixed_plan: " + _err())
+    first = {int(cls[j]): j for j in reversed(range(k))}          # a member of each class
+    kernels = [("neuron" if neuron[c] else "lane") if is_float[first[c]] else "int8" for c in range(r)]
+    return int(spc.value), [int(cls[j]) for j in range(k)], [(kernels[c], int(ctas[c])) for c in range(r)]
+
+
 class Group:
     """The synthesize / decode calls of several Batch objects of one flavour (all int8 or all float) and one GRU_A size on one
     device as one call: one per-sample launch for all their streams (lpcnet_b200_group_*).  Group stream rows = batches[0]'s
@@ -801,6 +836,71 @@ class MultiGroup:
             return self._gathered(call, pcm)
         call(None)
         return pcm
+
+
+class MixedGroup:
+    """Batch objects of any GRU_A sizes and flavours on one device served by one call: one group per (GRU_A size, flavour) class,
+    all planned together so that they fit on the SMs at once, each class's launches on a CUDA stream of its own
+    (lpcnet_b200_mixed_group_*).  Rows = batches[0]'s streams, then batches[1]'s, ...
+    The members stay usable on their own; the mixed group keeps them alive and must be closed before they are."""
+
+    def __init__(self, batches):
+        self._L = lib()
+        self.batches = list(batches)
+        hs = (c_p * max(len(self.batches), 1))(*[b._h if b is not None else None for b in self.batches])
+        self._h = self._L.lpcnet_b200_mixed_group_create(hs if self.batches else None, len(self.batches))
+        if not self._h:
+            raise LPCNetB200Error("lpcnet_b200_mixed_group_create: " + _err())
+        self.n = int(self._L.lpcnet_b200_mixed_group_streams(self._h))
+        self.classes = int(self._L.lpcnet_b200_mixed_group_classes(self._h))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.lpcnet_b200_mixed_group_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def group(self, c):
+        """class c's group (last_sample_kernel_ms of its part of the last call)"""
+        h = self._L.lpcnet_b200_mixed_group_group(self._h, int(c))
+        if not h:
+            raise LPCNetB200Error(_err())
+        return _OwnedGroup(h, self)
+
+    def synthesize(self, features, samples_per_frame=160):
+        """features [sum n][T][stride>=20] float32 (host) -> pcm [sum n][T*samples_per_frame] int16 (host)."""
+        f = np.ascontiguousarray(features, dtype=np.float32)
+        if f.ndim != 3 or f.shape[0] != self.n:
+            raise LPCNetB200Error("mixed_group synthesize: features of shape %s for %d streams" % (f.shape, self.n))
+        T, stride = f.shape[1], f.shape[2]
+        pcm = np.zeros((self.n, T * samples_per_frame), dtype=np.int16)
+        if self._L.lpcnet_b200_mixed_group_synthesize(self._h, f.ctypes.data, T, stride, samples_per_frame, pcm.ctypes.data) != 0:
+            raise LPCNetB200Error("lpcnet_b200_mixed_group_synthesize: " + _err())
+        return pcm
+
+    def synthesize_device(self, d_features_ptr, nframes, stride, d_pcm_ptr, samples_per_frame=160, cuda_stream=None):
+        if self._L.lpcnet_b200_mixed_group_synthesize_device(self._h, d_features_ptr, nframes, stride, samples_per_frame, d_pcm_ptr,
+                                                             cuda_stream) != 0:
+            raise LPCNetB200Error("lpcnet_b200_mixed_group_synthesize_device: " + _err())
+
+    def decode(self, packets):
+        """packets [sum n][P][8] uint8 -> pcm [sum n][P*640] int16."""
+        p = np.ascontiguousarray(packets, dtype=np.uint8)
+        if p.ndim != 3 or p.shape[0] != self.n or p.shape[2] != 8:
+            raise LPCNetB200Error("mixed_group decode: packets of shape %s for %d streams" % (p.shape, self.n))
+        pcm = np.zeros((self.n, p.shape[1] * 640), dtype=np.int16)
+        if self._L.lpcnet_b200_mixed_group_decode(self._h, p.ctypes.data, p.shape[1], pcm.ctypes.data) != 0:
+            raise LPCNetB200Error("lpcnet_b200_mixed_group_decode: " + _err())
+        return pcm
+
+    def decode_device(self, d_packets_ptr, npackets, d_pcm_ptr, cuda_stream=None):
+        if self._L.lpcnet_b200_mixed_group_decode_device(self._h, d_packets_ptr, npackets, d_pcm_ptr, cuda_stream) != 0:
+            raise LPCNetB200Error("lpcnet_b200_mixed_group_decode_device: " + _err())
+
+    def last_call_ms(self):
+        """device time of the last call, fork to join"""
+        return float(self._L.lpcnet_b200_mixed_group_last_call_ms(self._h))
 
 
 class LPCNet:

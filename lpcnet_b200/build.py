@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "liblpcnet_b200.so")
-HOST_SOURCES = ["model.cu", "frame_kernels.cu", "batch_api.cu", "lpcnet_api.cu", "microbench.cu", "multi_api.cu", "blob_io.cu", "enc_kernels.cu"]
+HOST_SOURCES = ["model.cu", "frame_kernels.cu", "batch_api.cu", "lpcnet_api.cu", "microbench.cu", "multi_api.cu", "mixed_api.cu", "blob_io.cu", "enc_kernels.cu"]
 KERNEL_SOURCES = ["sample_kernel.cu", "sample_kernel_f32.cu", "sample_kernel_f32n.cu"]   # compiled once per GRU_A size (-DLPCNET_NA=<na>, engine.h)
 NA_SIZES = [128, 256, 384]
 HOST_SOURCES = [f for f in HOST_SOURCES if os.path.exists(os.path.join(CSRC, f))]

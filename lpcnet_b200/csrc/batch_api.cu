@@ -876,13 +876,23 @@ int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_
 // The float flavour takes spc from group_plan and then the kernel a batch would (launch_sample): at spc <= FN_S, unless
 // LPCNET_B200_FLOAT_LANE_STREAM is set, the neuron-per-lane kernel, whose CTAs lay out S = 1, 2 or FN_S streams (spc 3 -> 4);
 // otherwise the lane == stream kernel with spc.  Member k takes ceil(n_k / slots) CTAs.  Returns true for the neuron-per-lane kernel.
+static int float_slots(int spc, bool lane_stream, bool *neuron)
+{
+    *neuron = spc <= FN_S && !lane_stream;
+    return !*neuron ? spc : spc <= 1 ? 1 : spc == 2 ? 2 : FN_S;
+}
+static int plan_ctas(const int *n, int count, int slots)
+{
+    int c = 0;
+    for (int k = 0; k < count; k++) c += (n[k] + slots - 1) / slots;
+    return c;
+}
 static bool group_plan_float(const int *n, int count, int sms, int override_spc, bool lane_stream, int *spc, int *slots, int *ctas)
 {
+    bool neuron;
     *spc = group_plan(n, count, sms, override_spc, ctas);
-    const bool neuron = *spc <= FN_S && !lane_stream;
-    *slots = !neuron ? *spc : *spc <= 1 ? 1 : *spc == 2 ? 2 : FN_S;
-    *ctas = 0;
-    for (int k = 0; k < count; k++) *ctas += (n[k] + *slots - 1) / *slots;
+    *slots = float_slots(*spc, lane_stream, &neuron);
+    *ctas = plan_ctas(n, count, *slots);
     return neuron;
 }
 
@@ -891,6 +901,23 @@ int lpcnet_b200_debug_group_plan_float(const int *n, int count, int sms, int ove
     if (!n || count < 1 || count > GROUP_MAX || sms < 1 || !spc || !slots || !ctas) { set_error("debug_group_plan_float: bad arguments"); return -1; }
     for (int k = 0; k < count; k++) if (n[k] < 1) { set_error("debug_group_plan_float: member %d has no streams", k); return -1; }
     return group_plan_float(n, count, sms, override_spc, lane_stream != 0, spc, slots, ctas) ? 1 : 0;
+}
+
+int lpcnet_b200_debug_mixed_plan(const int *n, const int *na, const int *is_float, int count, int sms, int override_spc, int lane_stream,
+                                 int *spc, int *class_of, int *class_ctas, int *class_neuron)
+{
+    if (!n || !na || !is_float || count < 1 || count > GROUP_MAX || sms < 1 || !spc || !class_of || !class_ctas || !class_neuron) {
+        set_error("debug_mixed_plan: bad arguments"); return -1;
+    }
+    for (int k = 0; k < count; k++) {
+        if (n[k] < 1) { set_error("debug_mixed_plan: member %d has no streams", k); return -1; }
+        if (!na_supported(na[k])) { set_error("debug_mixed_plan: member %d has %d GRU_A units (128, 256 or 384)", k, na[k]); return -1; }
+        if (is_float[k] != 0 && is_float[k] != 1) { set_error("debug_mixed_plan: member %d: is_float must be 0 or 1", k); return -1; }
+    }
+    bool neuron[GROUP_MAX];
+    const int classes = mixed_plan(n, na, is_float, count, sms, override_spc, lane_stream != 0, spc, class_of, class_ctas, neuron);
+    for (int c = 0; c < classes; c++) class_neuron[c] = neuron[c] ? 1 : 0;
+    return classes;
 }
 
 void lpcnet_b200_group_destroy(LPCNetB200Group *g)
@@ -907,45 +934,11 @@ void lpcnet_b200_group_destroy(LPCNetB200Group *g)
 
 LPCNetB200Group *lpcnet_b200_group_create(LPCNetB200Batch *const *batches, int count)
 {
-    if (!batches || count < 1 || count > GROUP_MAX) { set_error("group_create: 1..%d member batches", GROUP_MAX); return nullptr; }
-    for (int k = 0; k < count; k++) {
-        const LPCNetB200Batch *b = batches[k];
-        if (!b) { set_error("group_create: member %d is NULL", k); return nullptr; }
-        if (b->model.is_float != batches[0]->model.is_float) {
-            set_error("group_create: member %d holds %s model, member 0 %s one; the members of a group are all int8 or all float", k,
-                      b->model.is_float ? "a float" : "an int8", batches[0]->model.is_float ? "a float" : "an int8");
-            return nullptr;
-        }
-        if (b->device != batches[0]->device) { set_error("group_create: member %d is on device %d, member 0 on device %d", k, b->device, batches[0]->device); return nullptr; }
-        if (b->model.na != batches[0]->model.na) { set_error("group_create: member %d has %d GRU_A units, member 0 has %d", k, b->model.na, batches[0]->model.na); return nullptr; }
-        for (int j = 0; j < k; j++) if (batches[j] == b) { set_error("group_create: member %d is listed twice (also member %d)", k, j); return nullptr; }
-    }
-    if (cudaSetDevice(batches[0]->device) != cudaSuccess) { set_error("group_create: cudaSetDevice(%d) failed", batches[0]->device); return nullptr; }
-    LPCNetB200Group *g = new LPCNetB200Group();
-    g->count = count; g->device = batches[0]->device; g->na = batches[0]->model.na;
-    g->is_float = batches[0]->model.is_float != 0;
-    g->fast_cvt = true;
-    int n[GROUP_MAX];
-    for (int k = 0; k < count; k++) {
-        LPCNetB200Batch *b = batches[k];
-        g->m[k] = b; n[k] = b->n; g->n_total += b->n;
-        g->fast_cvt = g->fast_cvt && batch_fast_cvt(b);
-    }
-    int dev = g->device, sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    if (group_members_check(batches, count, "group_create", true)) return nullptr;
+    int n[GROUP_MAX], ctas;
+    for (int k = 0; k < count; k++) n[k] = batches[k]->n;
     const char *e = getenv("LPCNET_B200_STREAMS_PER_CTA");
-    if (g->is_float) {
-        g->neuron = group_plan_float(n, count, sms, e ? atoi(e) : 0, getenv("LPCNET_B200_FLOAT_LANE_STREAM") != nullptr, &g->spc, &g->slots, &g->ctas);
-    } else {
-        g->spc = group_plan(n, count, sms, e ? atoi(e) : 0, &g->ctas);
-        g->slots = g->spc;
-    }
-    for (int k = 0; k < count; k++)      // the footprint of the layout the chosen kernel uses
-        g->smem_bytes = std::max(g->smem_bytes, g->neuron ? batches[k]->model.Ln.total_bytes : batches[k]->model.L.total_bytes);
-    if (cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        set_error("group_create: cudaStreamCreate failed"); lpcnet_b200_group_destroy(g); return nullptr;
-    }
-    return g;
+    return group_init(batches, count, group_plan(n, count, device_sms(batches[0]->device), e ? atoi(e) : 0, &ctas));
 }
 
 int lpcnet_b200_group_streams(const LPCNetB200Group *g) { return g ? g->n_total : 0; }
@@ -1035,15 +1028,6 @@ static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_s
     return 0;
 }
 
-static int group_check(LPCNetB200Group *g)
-{
-    if (!g) { set_error("null group"); return -1; }
-    for (int k = 0; k < g->count; k++)
-        if (g->m[k]->sink) { set_error("group call: member %d has a PCM sink set; groups do not forward PCM to sinks", k); return -1; }
-    CK(cudaSetDevice(g->device));
-    return 0;
-}
-
 int lpcnet_b200_group_synthesize_device(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride,
                                         int samples_per_frame, short *d_pcm, void *cuda_stream)
 {
@@ -1112,6 +1096,97 @@ static int group_decode(LPCNetB200Group *g, const uint8_t *const *packets, int n
 }
 
 }  // extern "C"
+
+// ---- the parts of group_create that mixed groups share (engine.h) ----
+int lpcnet_b200::group_members_check(LPCNetB200Batch *const *batches, int count, const char *who, bool one_shape)
+{
+    if (!batches || count < 1 || count > GROUP_MAX) { set_error("%s: 1..%d member batches", who, GROUP_MAX); return -1; }
+    for (int k = 0; k < count; k++) {
+        const LPCNetB200Batch *b = batches[k];
+        if (!b) { set_error("%s: member %d is NULL", who, k); return -1; }
+        if (one_shape && b->model.is_float != batches[0]->model.is_float) {
+            set_error("%s: member %d holds %s model, member 0 %s one; the members of a group are all int8 or all float", who, k,
+                      b->model.is_float ? "a float" : "an int8", batches[0]->model.is_float ? "a float" : "an int8");
+            return -1;
+        }
+        if (b->device != batches[0]->device) { set_error("%s: member %d is on device %d, member 0 on device %d", who, k, b->device, batches[0]->device); return -1; }
+        if (one_shape && b->model.na != batches[0]->model.na) { set_error("%s: member %d has %d GRU_A units, member 0 has %d", who, k, b->model.na, batches[0]->model.na); return -1; }
+        for (int j = 0; j < k; j++) if (batches[j] == b) { set_error("%s: member %d is listed twice (also member %d)", who, k, j); return -1; }
+    }
+    return 0;
+}
+
+int lpcnet_b200::device_sms(int device)
+{
+    int sms = 0;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 132;
+    return sms;
+}
+
+int lpcnet_b200::batch_device(const LPCNetB200Batch *b) { return b->device; }
+
+LPCNetB200Group *lpcnet_b200::group_init(LPCNetB200Batch *const *batches, int count, int spc)
+{
+    if (cudaSetDevice(batches[0]->device) != cudaSuccess) { set_error("group_create: cudaSetDevice(%d) failed", batches[0]->device); return nullptr; }
+    LPCNetB200Group *g = new LPCNetB200Group();
+    g->count = count; g->device = batches[0]->device; g->na = batches[0]->model.na;
+    g->is_float = batches[0]->model.is_float != 0;
+    g->fast_cvt = true;
+    int n[GROUP_MAX];
+    for (int k = 0; k < count; k++) {
+        LPCNetB200Batch *b = batches[k];
+        g->m[k] = b; n[k] = b->n; g->n_total += b->n;
+        g->fast_cvt = g->fast_cvt && batch_fast_cvt(b);
+    }
+    g->spc = spc;
+    g->slots = g->is_float ? float_slots(spc, getenv("LPCNET_B200_FLOAT_LANE_STREAM") != nullptr, &g->neuron) : spc;
+    g->ctas = plan_ctas(n, count, g->slots);
+    for (int k = 0; k < count; k++)      // the footprint of the layout the chosen kernel uses
+        g->smem_bytes = std::max(g->smem_bytes, g->neuron ? batches[k]->model.Ln.total_bytes : batches[k]->model.L.total_bytes);
+    if (cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) != cudaSuccess) {
+        set_error("group_create: cudaStreamCreate failed"); lpcnet_b200_group_destroy(g); return nullptr;
+    }
+    return g;
+}
+
+int lpcnet_b200::mixed_plan(const int *n, const int *na, const int *is_float, int count, int sms, int override_spc, bool lane_stream,
+                            int *spc, int *class_of, int *class_ctas, bool *class_neuron)
+{
+    int ctas, classes = 0, cls_na[GROUP_MAX], cls_float[GROUP_MAX], slots[GROUP_MAX];
+    *spc = group_plan(n, count, sms, override_spc, &ctas);
+    for (int k = 0; k < count; k++) {
+        int c = 0;
+        while (c < classes && (cls_na[c] != na[k] || cls_float[c] != is_float[k])) c++;
+        if (c == classes) {
+            cls_na[c] = na[k]; cls_float[c] = is_float[k]; class_ctas[c] = 0; class_neuron[c] = false;
+            slots[c] = is_float[k] ? float_slots(*spc, lane_stream, &class_neuron[c]) : *spc;
+            classes++;
+        }
+        class_of[k] = c;
+        class_ctas[c] += (n[k] + slots[c] - 1) / slots[c];
+    }
+    return classes;
+}
+
+int lpcnet_b200::group_check(LPCNetB200Group *g)
+{
+    if (!g) { set_error("null group"); return -1; }
+    for (int k = 0; k < g->count; k++)
+        if (g->m[k]->sink) { set_error("group call: member %d has a PCM sink set; groups do not forward PCM to sinks", k); return -1; }
+    CK(cudaSetDevice(g->device));
+    return 0;
+}
+
+int lpcnet_b200::group_synthesize_members(LPCNetB200Group *g, const float *const *feat, int nframes, int feature_stride, int spf,
+                                          short *const *pcm, cudaStream_t st)
+{
+    return group_synth(g, feat, feature_stride, nframes, spf, pcm, nullptr, st);
+}
+
+int lpcnet_b200::group_decode_members(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, cudaStream_t st)
+{
+    return group_decode(g, packets, npackets, pcm, nullptr, st);
+}
 
 // ---- the entries of the multi-GPU groups (engine.h) ----
 int lpcnet_b200::group_call_check(const LPCNetB200Group *g, int nframes, int frame_stride, int spf, bool decode)

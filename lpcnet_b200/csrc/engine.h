@@ -421,3 +421,28 @@ int group_synthesize_forward(LPCNetB200Group *g, const float *d_features, int nf
                              const PcmTarget *fwd, cudaStream_t st);
 int group_decode_forward(LPCNetB200Group *g, const uint8_t *d_packets, int npackets, short *d_pcm, const PcmTarget *fwd, cudaStream_t st);
 }  // namespace lpcnet_b200
+
+// ---- the parts of groups that mixed groups (mixed_api.cu) are built from (batch_api.cu) ----
+struct LPCNetB200Batch;
+namespace lpcnet_b200 {
+// 1..GROUP_MAX batches, none NULL, none listed twice, all on one device; with one_shape also one GRU_A size and one flavour.
+// Otherwise sets the error (prefixed with `who`) and returns -1.
+int group_members_check(LPCNetB200Batch *const *batches, int count, const char *who, bool one_shape);
+// The group over checked one-shape members at `spc` streams per CTA: kernel, slots, CTAs and shared memory follow from spc as
+// lpcnet_b200_group_create picks them (LPCNET_B200_FLOAT_LANE_STREAM read here).  NULL (error set) on failure.
+LPCNetB200Group *group_init(LPCNetB200Batch *const *batches, int count, int spc);
+int device_sms(int device);                   // SM count (132 if the query fails)
+int batch_device(const LPCNetB200Batch *b);
+// The plan of a mixed group (lpcnet_b200_debug_mixed_plan, checked arguments): members are classed by (na, is_float) in order of
+// first appearance; spc is what a group over ALL members would plan; class c takes the CTAs its group takes at that spc.
+// Returns the number of classes.
+int mixed_plan(const int *n, const int *na, const int *is_float, int count, int sms, int override_spc, bool lane_stream,
+               int *spc, int *class_of, int *class_ctas, bool *class_neuron);
+// What a public group call refuses before its arguments: a member with a PCM sink (also sets the group's device)
+int group_check(LPCNetB200Group *g);
+// The group's synthesize / decode `_device` calls with member k's inputs at feat[k] / packets[k] and its PCM at pcm[k]
+// ([n_k][nframes*spf] resp. [n_k][npackets*640]), everything on `st`; no sink check (group_check) and no forwarding.
+int group_synthesize_members(LPCNetB200Group *g, const float *const *feat, int nframes, int feature_stride, int spf,
+                             short *const *pcm, cudaStream_t st);
+int group_decode_members(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, cudaStream_t st);
+}  // namespace lpcnet_b200
