@@ -35,6 +35,45 @@ struct CondFrame { float *A, *B, *L; };
 // device buffers of a copy of the per-stream state (a batch's shadow copy, a snapshot), for the parts it was allocated for
 struct StateCopy { SampleState ss; FrameState fs; CondFrame tail; };
 
+// Chunks of PCM forwarded to PcmTargets (a batch's sink, the gather buffer of a multi-GPU group) on a copy stream that overlaps
+// the next chunk's kernels; the stream is made on first use
+struct PcmForwarder {
+    cudaStream_t stream; cudaEvent_t ev, done;     // ev: the copy stream's hand-over event
+    int open()
+    {
+        if (stream) return 0;
+        CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+        CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+        return 0;
+    }
+    // chunk [c0, c0+nf) of the n PCM rows at d_pcm is complete on `st`: its block goes to t
+    int forward_to_sink(const PcmTarget &t, int n, const short *d_pcm, long long pcm_stride, int c0, int nf, int spf, cudaStream_t st)
+    {
+        CK(cudaEventRecord(ev, st));
+        CK(cudaStreamWaitEvent(stream, ev, 0));
+        short *dst = t.dst + t.row0 * t.pitch + (size_t)c0 * spf;
+        if (c0 == 0 && (long long)nf * spf == pcm_stride && t.pitch == pcm_stride)      // whole rows, same pitch: one contiguous block (one DMA descriptor
+            CK(cudaMemcpyAsync(dst, d_pcm, (size_t)n * pcm_stride * sizeof(short), cudaMemcpyDefault, stream));   // instead of n row copies)
+        else
+            CK(cudaMemcpy2DAsync(dst, t.pitch * sizeof(short), d_pcm + (size_t)c0 * spf, pcm_stride * sizeof(short), (size_t)nf * spf * sizeof(short), n,
+                                 cudaMemcpyDefault, stream));       // (the target may live on another device: UVA infers the route)
+        return 0;
+    }
+    int join(cudaStream_t st)        // the call's stream also waits for the forwarded copies: "call complete" includes "PCM at the target"
+    {
+        CK(cudaEventRecord(done, stream));
+        CK(cudaStreamWaitEvent(st, done, 0));
+        return 0;
+    }
+    void destroy()
+    {
+        if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+        if (ev) cudaEventDestroy(ev);
+        if (done) cudaEventDestroy(done);
+    }
+};
+
 struct LPCNetB200Batch {
     int device, n;
     DeviceModel model;
@@ -65,22 +104,26 @@ struct LPCNetB200Batch {
     std::vector<cudaEvent_t> kev;                 // event pairs around every per-sample kernel launch of the last call
     int kev_used;
     int last_launches;
-    // PCM sink (multi-GPU gather): after every chunk the chunk's PCM block is also copied, on a copy stream that overlaps the next
-    // chunk's kernels, to sink + row0*pitch (a buffer of another device / another process opened through CUDA IPC)
-    short *sink; long long sink_pitch; long long sink_row0; cudaStream_t sink_stream; cudaEvent_t sink_ev, sink_done;
+    // PCM sink (multi-GPU gather): after every chunk the chunk's PCM block is also forwarded to the sink (a buffer of another
+    // device / another process opened through CUDA IPC)
+    PcmTarget sink; PcmForwarder fwd;
 };
 
-static int order_sync(LPCNetB200Batch *b);
-// grow a staging buffer; work on any stream may still be using the old one, so wait for it before freeing
-static int ensure(LPCNetB200Batch *b, void **p, size_t *cap, size_t bytes)
+int lpcnet_b200::grow_buffer(void **p, size_t *cap, size_t bytes)
 {
     if (*cap >= bytes) return 0;
-    if (order_sync(b)) return -1;
     if (*p) cudaFree(*p);
     *p = nullptr; *cap = 0;
     CK(cudaMalloc(p, bytes));
     *cap = bytes;
     return 0;
+}
+static int order_sync(LPCNetB200Batch *b);
+// grow a staging buffer; work on any stream may still be using the old one, so wait for it before freeing
+static int ensure(LPCNetB200Batch *b, void **p, size_t *cap, size_t bytes)
+{
+    if (*cap >= bytes) return 0;
+    return order_sync(b) || grow_buffer(p, cap, bytes) ? -1 : 0;
 }
 
 // stream hand-over (see LPCNetB200Batch::order_ev)
@@ -122,16 +165,26 @@ static int probe_smem_base(uint32_t *base)
     return 0;
 }
 
-// Live streams per CTA: a batch smaller than 32 x SM count is spread over all SMs (one CTA per SM, fewer live slots each)
-// instead of filling a few SMs completely: the time of a CTA-step barely depends on how many of its slots are live.
-int lpcnet_b200::streams_per_cta_for(int n_streams, int override_spc)
+// The launch plan of a batch (one member) and of a group.  Live streams per CTA: a job smaller than 32 x SM count is spread over
+// all SMs (fewer live slots per CTA) instead of filling a few SMs completely: the time of a CTA-step barely depends on how many of
+// its slots are live.  One streams-per-CTA value for the whole launch: the smallest that puts every member on at most `sms` CTAs in
+// total, member k on ceil(n_k / spc) CTAs of its own; 32 when none does (LPCNET_B200_STREAMS_PER_CTA overrides it, clamped to 32).
+static int group_plan(const int *n, int count, int sms, int override_spc, int *ctas)
 {
-    // (spc <= 16 additionally selects the half-A-only schedule)
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    int spc = (n_streams + sms - 1) / sms;
-    if (override_spc > 0) spc = override_spc;                    // LPCNET_B200_STREAMS_PER_CTA, read once per batch at create time (tests, tuning)
-    return spc < 1 ? 1 : spc > STREAMS_PER_CTA ? STREAMS_PER_CTA : spc;
+    auto total = [&](int spc) { int c = 0; for (int k = 0; k < count; k++) c += (n[k] + spc - 1) / spc; return c; };
+    int spc = STREAMS_PER_CTA;
+    if (override_spc > 0) spc = std::min(override_spc, STREAMS_PER_CTA);
+    else for (int s = 1; s <= STREAMS_PER_CTA; s++) if (total(s) <= sms) { spc = s; break; }
+    *ctas = total(spc);
+    return spc;
+}
+// The float flavour takes spc from group_plan and then its kernel: at spc <= FN_S, unless LPCNET_B200_FLOAT_LANE_STREAM is set,
+// the neuron-per-lane kernel, whose CTAs lay out S = 1, 2 or FN_S streams (spc 3 -> 4); otherwise the lane == stream kernel with
+// spc.  Returns the streams a CTA lays out (member k takes ceil(n_k / slots) CTAs); *neuron: the neuron-per-lane kernel.
+static int float_slots(int spc, bool lane_stream, bool *neuron)
+{
+    *neuron = spc <= FN_S && !lane_stream;
+    return !*neuron ? spc : spc <= 1 ? 1 : spc == 2 ? 2 : FN_S;
 }
 int lpcnet_b200::sample_kernel_smem_ok(uint32_t bytes) { return bytes <= 227u * 1024u; }
 
@@ -405,9 +458,7 @@ void lpcnet_b200_batch_destroy(LPCNetB200Batch *b)
     if (b->fs.side) { cudaStreamSynchronize(b->fs.side); cudaStreamDestroy(b->fs.side); }
     if (b->fs.ev_fork) cudaEventDestroy(b->fs.ev_fork);
     if (b->fs.ev_join) cudaEventDestroy(b->fs.ev_join);
-    if (b->sink_stream) { cudaStreamSynchronize(b->sink_stream); cudaStreamDestroy(b->sink_stream); }
-    if (b->sink_ev) cudaEventDestroy(b->sink_ev);
-    if (b->sink_done) cudaEventDestroy(b->sink_done);
+    b->fwd.destroy();
     free_state(batch_fields(b, -1)); free_state(shadow_fields(b));
     void *ptrs[] = {b->fs.work, b->condA, b->condB, b->lpc_raw, b->d_features, b->d_pcm, b->d_packets, b->d_state, b->d_mask};
     for (void *p : ptrs) if (p) cudaFree(p);
@@ -489,15 +540,17 @@ static int launch_sample(LPCNetB200Batch *b, int pos, int nf, int spf, short *pc
 {
     const int n = b->n, na = b->model.na;
     SampleParams p = sample_params(b, pos, nf, spf, pcm, pcm_stride);
-    p.spc = streams_per_cta_for(n, b->env_spc);
+    int ctas;
+    bool small_float = false;       // small batch: the neuron-per-lane float kernel
+    p.spc = group_plan(&n, 1, device_sms(b->device), b->env_spc, &ctas);
+    if (b->model.is_float) float_slots(p.spc, b->env_float_lane_stream, &small_float);
     p.one_half = p.spc <= HALF && !b->env_two_halves;
     p.fast_cvt = (batch_fast_cvt(b) ? 1 : 0) | (preload << 8);
 #ifdef LPCNET_TRACE
     { static long long *d_trace = nullptr; if (!d_trace) { CK(cudaMalloc(&d_trace, (8 * 32 + 8 * 32 * 16) * 8)); CK(cudaMemset(d_trace, 0, (8 * 32 + 8 * 32 * 16) * 8)); } p.trace = d_trace; g_trace = d_trace; }
 #endif
     if (time_it && time_launch(b->kev, &b->kev_used, st)) return -1;
-    const bool small_float = b->model.is_float && p.spc <= FN_S && !b->env_float_lane_stream;
-    if (small_float) { p.L = b->model.Ln; p.image = b->model.image_n; }       // small batch: neuron-per-lane float kernel
+    if (small_float) { p.L = b->model.Ln; p.image = b->model.image_n; }
     cudaError_t e;
 #define LPCNET_DISPATCH(ns) (small_float ? ns::launch_sample_kernel_f32n(p, st) : b->model.is_float ? ns::launch_sample_kernel_f32(p, st) : ns::launch_sample_kernel(p, st))
     switch (na) {
@@ -547,39 +600,22 @@ static int sample_prefix(LPCNetB200Batch *b, int pos0, int nf, int spf, short *p
     *live0 = sil_any;
     return launches;
 }
+// the launch that ends a batch's chunk: frames [live0, nf) of the frames at chunk positions [pos0, pos0 + nf), if any are left.
+// Returns the number of engine kernels launched, < 0 on error.
+static int launch_rest(LPCNetB200Batch *b, int pos0, int live0, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st)
+{
+    if (nf <= live0) return 0;
+    return launch_sample(b, pos0 + live0, nf - live0, spf, pcm + (size_t)live0 * spf, pcm_stride, live0 == 0 ? preload : 0, st, true) ? -1 : 1;
+}
 static int sample_frames(LPCNetB200Batch *b, int pos0, int nf, int spf, short *pcm, long long pcm_stride, int preload, cudaStream_t st)
 {
     int sil_any = 0;
     int launches = sample_prefix(b, pos0, nf, spf, pcm, pcm_stride, preload, st, &sil_any);
     if (launches < 0) return -1;
-    if (nf > sil_any) {
-        if (launch_sample(b, pos0 + sil_any, nf - sil_any, spf, pcm + (size_t)sil_any * spf, pcm_stride, sil_any == 0 ? preload : 0, st, true)) return -1;
-        launches += 1;
-    }
+    const int r = launch_rest(b, pos0, sil_any, nf, spf, pcm, pcm_stride, preload, st);
+    if (r < 0) return -1;
     for (int &v : b->fc) v = std::min(1000, v + nf);
-    return launches;
-}
-
-// chunk [c0, c0+nf) of the n PCM rows at d_pcm is complete on `st`: forward its block to target t on the copy stream `cs`, which
-// overlaps the next chunk's kernels (`ev`: the copy stream's hand-over event)
-static int forward_chunk(const PcmTarget &t, int n, const short *d_pcm, long long pcm_stride, int c0, int nf, int spf, cudaStream_t st,
-                         cudaStream_t cs, cudaEvent_t ev)
-{
-    CK(cudaEventRecord(ev, st));
-    CK(cudaStreamWaitEvent(cs, ev, 0));
-    short *dst = t.dst + t.row0 * t.pitch + (size_t)c0 * spf;
-    if (c0 == 0 && (long long)nf * spf == pcm_stride && t.pitch == pcm_stride)      // whole rows, same pitch: one contiguous block (one DMA descriptor
-        CK(cudaMemcpyAsync(dst, d_pcm, (size_t)n * pcm_stride * sizeof(short), cudaMemcpyDefault, cs));   // instead of n row copies)
-    else
-        CK(cudaMemcpy2DAsync(dst, t.pitch * sizeof(short), d_pcm + (size_t)c0 * spf, pcm_stride * sizeof(short), (size_t)nf * spf * sizeof(short), n,
-                             cudaMemcpyDefault, cs));       // (the target may live on another device: UVA infers the route)
-    return 0;
-}
-// ... to the batch's sink, if one is set
-static int forward_to_sink(LPCNetB200Batch *b, const short *d_pcm, long long pcm_stride, int c0, int nf, int spf, cudaStream_t st)
-{
-    if (!b->sink) return 0;
-    return forward_chunk(PcmTarget{b->sink, b->sink_pitch, b->sink_row0}, b->n, d_pcm, pcm_stride, c0, nf, spf, st, b->sink_stream, b->sink_ev);
+    return launches + r;
 }
 
 // The 100 Hz part of a chunk [c0, c0 + nf) of a call: the frame network on the batch's rows of the features; the chunk's last
@@ -591,36 +627,20 @@ static int frame_chunk(LPCNetB200Batch *b, const float *d_feat, long long stream
     return frame_network_launches(b->model);
 }
 
-// Core: features and pcm are device pointers. `st` is the stream all work is enqueued on.
-static int synth_device(LPCNetB200Batch *b, const float *d_feat, long long stream_stride, int frame_stride, int nframes,
-                        int spf, short *d_pcm, int preload, cudaStream_t st)
+static int run_call(LPCNetB200Group *g, LPCNetB200Batch *b, const CallShape &c, const void *const *in, short *const *pcm, const PcmTarget *fwd,
+                    int preload, cudaStream_t st);
+// A batch call on device buffers: features or packets at d_in, PCM at d_pcm, everything on `st`
+static int batch_call(LPCNetB200Batch *b, const CallShape &c, const void *d_in, short *d_pcm, int preload, cudaStream_t st)
 {
     if (!b) { set_error("null batch"); return -1; }
-    if (nframes <= 0) return 0;
-    if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
-    if (preload < 0 || preload > spf) { set_error("preload must be in 0..samples_per_frame"); return -1; }
-    if (frame_stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
-    const long long pcm_stride = (long long)nframes * spf;
-    if (b->sink && b->sink_pitch < pcm_stride) { set_error("PCM sink pitch %lld smaller than the call's %lld samples per stream", b->sink_pitch, pcm_stride); return -1; }
-    int launches = 0;
-    b->kev_used = 0;
-    if (order_enter(b, st)) return -1;
-    for (int c0 = 0; c0 < nframes; c0 += CHUNK) {
-        const int nf = nframes - c0 < CHUNK ? nframes - c0 : CHUNK;
-        launches += frame_chunk(b, d_feat, stream_stride, frame_stride, c0, nf, st);
-        const int r = sample_frames(b, 0, nf, spf, d_pcm + (size_t)c0 * spf, pcm_stride, c0 == 0 ? preload : 0, st);
-        if (r < 0) return -1;
-        launches += r;
-        if (forward_to_sink(b, d_pcm, pcm_stride, c0, nf, spf, st)) return -1;
+    if (c.units <= 0) return 0;
+    if (c.check()) return -1;
+    if (preload < 0 || preload > c.spf) { set_error("preload must be in 0..samples_per_frame"); return -1; }
+    if (c.decode && !b->model.codebooks) { set_error("decode: no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)"); return -1; }
+    if (b->sink.dst && b->sink.pitch < c.pcm_samples()) {
+        set_error("PCM sink pitch %lld smaller than the call's %lld samples per stream", b->sink.pitch, c.pcm_samples()); return -1;
     }
-    CK(cudaGetLastError());
-    if (b->sink) {       // the call's stream also waits for the forwarded copies: "call complete" includes "PCM at the sink"
-        CK(cudaEventRecord(b->sink_done, b->sink_stream));
-        CK(cudaStreamWaitEvent(st, b->sink_done, 0));
-    }
-    if (order_leave(b, st)) return -1;
-    b->last_launches = launches;
-    return 0;
+    return run_call(nullptr, b, c, &d_in, &d_pcm, b->sink.dst ? &b->sink : nullptr, preload, st);
 }
 
 int lpcnet_b200_batch_synthesize_device_ex(LPCNetB200Batch *b, const float *d_features, int nframes, int feature_stride,
@@ -629,7 +649,7 @@ int lpcnet_b200_batch_synthesize_device_ex(LPCNetB200Batch *b, const float *d_fe
     if (!b) { set_error("null batch"); return -1; }
     CK(cudaSetDevice(b->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : b->stream;
-    int r = synth_device(b, d_features, (long long)nframes * feature_stride, feature_stride, nframes, samples_per_frame, d_pcm, preload, st);
+    int r = batch_call(b, CallShape::synthesis(nframes, feature_stride, samples_per_frame), d_features, d_pcm, preload, st);
     if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
     return r;
 }
@@ -646,17 +666,17 @@ int lpcnet_b200_batch_synthesize_ex(LPCNetB200Batch *b, const float *features, i
     if (nframes <= 0) return 0;
     if (!features || !pcm) { set_error("null buffer"); return -1; }
     CK(cudaSetDevice(b->device));
-    const size_t fbytes = sizeof(float) * (size_t)b->n * nframes * feature_stride;
-    const size_t pbytes = sizeof(short) * (size_t)b->n * nframes * samples_per_frame;
+    const CallShape c = CallShape::synthesis(nframes, feature_stride, samples_per_frame);
+    const size_t fbytes = c.in_bytes() * b->n, pbytes = sizeof(short) * c.pcm_samples() * b->n;
     if (ensure(b, (void **)&b->d_features, &b->d_features_cap, fbytes)) return -1;
     if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, pbytes)) return -1;
     if (order_enter(b, b->stream)) return -1;       // the staging buffers may still be read by work on another stream
     CK(cudaMemcpyAsync(b->d_features, features, fbytes, cudaMemcpyHostToDevice, b->stream));
     if (preload > 0)                                // teacher forcing reads the caller's signal from the output buffer (lpcnet.c:257)
-        CK(cudaMemcpy2DAsync(b->d_pcm, (size_t)nframes * samples_per_frame * sizeof(short), pcm, (size_t)nframes * samples_per_frame * sizeof(short),
+        CK(cudaMemcpy2DAsync(b->d_pcm, c.pcm_samples() * sizeof(short), pcm, c.pcm_samples() * sizeof(short),
                              (size_t)std::min(preload, samples_per_frame) * sizeof(short), b->n, cudaMemcpyHostToDevice, b->stream));
     if (order_leave(b, b->stream)) return -1;
-    if (synth_device(b, b->d_features, (long long)nframes * feature_stride, feature_stride, nframes, samples_per_frame, b->d_pcm, preload, b->stream)) return -1;
+    if (batch_call(b, c, b->d_features, b->d_pcm, preload, b->stream)) return -1;
     CK(cudaMemcpyAsync(pcm, b->d_pcm, pbytes, cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
     return 0;
@@ -682,9 +702,7 @@ int lpcnet_b200_batch_run_frame_network(LPCNetB200Batch *b, const float *feature
     CK(cudaMemcpyAsync(b->d_features, features, fbytes, cudaMemcpyHostToDevice, b->stream));
     for (int c0 = 0; c0 < nframes; c0 += CHUNK) {
         const int nf = std::min(CHUNK, nframes - c0);
-        launch_frame_network(b->model, b->fs, b->d_features + (size_t)c0 * feature_stride, (long long)nframes * feature_stride, feature_stride, b->n, nf,
-                             b->condA, b->condB, b->lpc_raw, b->stream);
-        b->cond_last = nf - 1;
+        frame_chunk(b, b->d_features, (long long)nframes * feature_stride, feature_stride, c0, nf, b->stream);
         for (int &v : b->fc) v = std::min(1000, v + nf);
     }
     if (order_leave(b, b->stream)) return -1;
@@ -785,26 +803,13 @@ int lpcnet_b200_batch_frame_network_flush(LPCNetB200Batch *b)
     return 0;
 }
 
-static int decode_device(LPCNetB200Batch *b, const uint8_t *d_packets, int npackets, short *d_pcm, cudaStream_t st)
-{
-    if (!b->model.codebooks) { set_error("decode: no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)"); return -1; }
-    const size_t fbytes = sizeof(float) * (size_t)b->n * npackets * 4 * NB_FEAT;
-    if (ensure(b, (void **)&b->d_features, &b->d_features_cap, fbytes)) return -1;
-    if (order_enter(b, st)) return -1;
-    launch_decode_packets(b->model, b->fs, d_packets, b->n, npackets, b->d_features, st);
-    if (order_leave(b, st)) return -1;
-    int r = synth_device(b, b->d_features, (long long)npackets * 4 * NB_FEAT, NB_FEAT, npackets * 4, FRAME_SIZE, d_pcm, 0, st);
-    b->last_launches += 1;
-    return r;
-}
-
 int lpcnet_b200_batch_decode_device(LPCNetB200Batch *b, const unsigned char *d_packets, int npackets, short *d_pcm, void *cuda_stream)
 {
     if (!b) { set_error("null batch"); return -1; }
     if (npackets <= 0) return 0;
     CK(cudaSetDevice(b->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : b->stream;
-    int r = decode_device(b, d_packets, npackets, d_pcm, st);
+    int r = batch_call(b, CallShape::packets(npackets), d_packets, d_pcm, 0, st);
     if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
     return r;
 }
@@ -815,13 +820,14 @@ int lpcnet_b200_batch_decode(LPCNetB200Batch *b, const unsigned char *packets, i
     if (npackets <= 0) return 0;
     if (!packets || !pcm) { set_error("null buffer"); return -1; }
     CK(cudaSetDevice(b->device));
-    const size_t kbytes = (size_t)b->n * npackets * 8, pbytes = sizeof(short) * (size_t)b->n * npackets * 640;
+    const CallShape c = CallShape::packets(npackets);
+    const size_t kbytes = c.in_bytes() * b->n, pbytes = sizeof(short) * c.pcm_samples() * b->n;
     if (ensure(b, (void **)&b->d_packets, &b->d_packets_cap, kbytes)) return -1;
     if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, pbytes)) return -1;
     if (order_enter(b, b->stream)) return -1;
     CK(cudaMemcpyAsync(b->d_packets, packets, kbytes, cudaMemcpyHostToDevice, b->stream));
     if (order_leave(b, b->stream)) return -1;
-    if (decode_device(b, b->d_packets, npackets, b->d_pcm, b->stream)) return -1;
+    if (batch_call(b, c, b->d_packets, b->d_pcm, 0, b->stream)) return -1;
     CK(cudaMemcpyAsync(pcm, b->d_pcm, pbytes, cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
     return 0;
@@ -837,8 +843,8 @@ float lpcnet_b200_batch_last_sample_kernel_ms(const LPCNetB200Batch *b, int *lau
 // ---- groups: the synthesize / decode calls of several batches of one flavour and GRU_A size on one device as one call ----
 // Each chunk runs every member's 100 Hz part and silent-frame prefix with the member's own launches, then ONE per-sample launch
 // for the frames that remain (GroupSampleParams; sample_kernel.cu, sample_kernel_f32.cu, sample_kernel_f32n.cu).  The members
-// keep all their state and host mirrors; the group only holds the launch plan, a stream for its host-pointer calls and the event
-// timers of its launches.
+// keep all their state and host mirrors; the group only holds the launch plan, a stream and staging for its host-pointer calls and
+// the event timers of its launches.
 struct LPCNetB200Group {
     int count, device, na, n_total;
     LPCNetB200Batch *m[GROUP_MAX];
@@ -850,20 +856,10 @@ struct LPCNetB200Group {
     cudaStream_t stream;
     std::vector<cudaEvent_t> kev;     // event pairs around the group's own per-sample launches of the last call
     int kev_used, last_launches;
-    cudaStream_t fwd_stream; cudaEvent_t fwd_ev, fwd_done;   // copy stream of the forwarded PCM (group_*_forward), made on first use
+    PcmForwarder fwd;                 // PCM forwarded to the targets of group_call
+    void *d_in; size_t d_in_cap;      // staging of the host-pointer calls
+    short *d_pcm; size_t d_pcm_cap;
 };
-
-// One streams-per-CTA value for the whole launch: the smallest that puts every member on at most `sms` CTAs in total, member k
-// on ceil(n_k / spc) CTAs of its own; 32 when none does.  A one-member group plans as streams_per_cta_for.
-static int group_plan(const int *n, int count, int sms, int override_spc, int *ctas)
-{
-    auto total = [&](int spc) { int c = 0; for (int k = 0; k < count; k++) c += (n[k] + spc - 1) / spc; return c; };
-    int spc = STREAMS_PER_CTA;
-    if (override_spc > 0) spc = std::min(override_spc, STREAMS_PER_CTA);
-    else for (int s = 1; s <= STREAMS_PER_CTA; s++) if (total(s) <= sms) { spc = s; break; }
-    *ctas = total(spc);
-    return spc;
-}
 
 int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_spc, int *spc, int *ctas)
 {
@@ -873,14 +869,6 @@ int lpcnet_b200_debug_group_plan(const int *n, int count, int sms, int override_
     return 0;
 }
 
-// The float flavour takes spc from group_plan and then the kernel a batch would (launch_sample): at spc <= FN_S, unless
-// LPCNET_B200_FLOAT_LANE_STREAM is set, the neuron-per-lane kernel, whose CTAs lay out S = 1, 2 or FN_S streams (spc 3 -> 4);
-// otherwise the lane == stream kernel with spc.  Member k takes ceil(n_k / slots) CTAs.  Returns true for the neuron-per-lane kernel.
-static int float_slots(int spc, bool lane_stream, bool *neuron)
-{
-    *neuron = spc <= FN_S && !lane_stream;
-    return !*neuron ? spc : spc <= 1 ? 1 : spc == 2 ? 2 : FN_S;
-}
 static int plan_ctas(const int *n, int count, int slots)
 {
     int c = 0;
@@ -925,9 +913,9 @@ void lpcnet_b200_group_destroy(LPCNetB200Group *g)
     if (!g) return;
     cudaSetDevice(g->device);
     if (g->stream) { cudaStreamSynchronize(g->stream); cudaStreamDestroy(g->stream); }
-    if (g->fwd_stream) { cudaStreamSynchronize(g->fwd_stream); cudaStreamDestroy(g->fwd_stream); }
-    if (g->fwd_ev) cudaEventDestroy(g->fwd_ev);
-    if (g->fwd_done) cudaEventDestroy(g->fwd_done);
+    g->fwd.destroy();
+    if (g->d_in) cudaFree(g->d_in);
+    if (g->d_pcm) cudaFree(g->d_pcm);
     for (cudaEvent_t e : g->kev) cudaEventDestroy(e);
     delete g;
 }
@@ -977,122 +965,121 @@ static int launch_group(LPCNetB200Group *g, const int *live0, int nf, int spf, s
     return 1;
 }
 
-// Core of the group calls: member k reads features feat[k] ([n_k][nframes][frame_stride]) and writes pcm[k] ([n_k][nframes*spf]),
-// all device pointers, everything on `st`.  Per chunk: every member's frame network, every member's silent prefix, one launch, and
-// the chunk's PCM forwarded to fwd[k] for the members that have a target (fwd NULL: none).
-static int group_synth(LPCNetB200Group *g, const float *const *feat, int frame_stride, int nframes, int spf, short *const *pcm,
-                       const PcmTarget *fwd, cudaStream_t st)
+// Core of the batch and group calls (g NULL: a call of batch b alone, with its preload; else of the group's members, preload 0).
+// Member k reads in[k] (features [n_k][frames][stride], or packets that are first decoded into the member's feature staging) and
+// writes pcm[k] ([n_k][frames * spf]), all device pointers, everything on `st`.  Per chunk: every member's frame network and
+// silent prefix, then the launch that ends the chunk (the batch's own, or one for the whole group), and the chunk's PCM forwarded
+// to fwd[k] for the members that have a target (fwd NULL: none).
+static int run_call(LPCNetB200Group *g, LPCNetB200Batch *b, const CallShape &c, const void *const *in, short *const *pcm, const PcmTarget *fwd,
+                    int preload, cudaStream_t st)
 {
-    if (nframes <= 0) return 0;
-    if (group_call_check(g, nframes, frame_stride, spf, false)) return -1;
-    const long long stream_stride = (long long)nframes * frame_stride, pcm_stride = (long long)nframes * spf;
-    bool forwarding = false;
-    for (int k = 0; fwd && k < g->count; k++) forwarding = forwarding || fwd[k].dst;
-    if (forwarding && !g->fwd_stream) {
-        CK(cudaStreamCreateWithFlags(&g->fwd_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&g->fwd_ev, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&g->fwd_done, cudaEventDisableTiming));
+    LPCNetB200Batch *const *m = g ? g->m : &b;
+    const int count = g ? g->count : 1, nframes = c.frames(), spf = c.spf;
+    const long long stream_stride = (long long)nframes * c.stride, pcm_stride = c.pcm_samples();
+    const float *feat[GROUP_MAX];
+    if (c.decode) {
+        for (int k = 0; k < count; k++)
+            if (ensure(m[k], (void **)&m[k]->d_features, &m[k]->d_features_cap, sizeof(float) * (size_t)m[k]->n * stream_stride)) return -1;
+        for (int k = 0; k < count; k++) {
+            if (order_enter(m[k], st)) return -1;
+            launch_decode_packets(m[k]->model, m[k]->fs, (const uint8_t *)in[k], m[k]->n, c.units, m[k]->d_features, st);
+            if (order_leave(m[k], st)) return -1;
+        }
     }
+    for (int k = 0; k < count; k++) feat[k] = c.decode ? m[k]->d_features : (const float *)in[k];
+    PcmForwarder &fw = g ? g->fwd : b->fwd;
+    bool forwarding = false;
+    for (int k = 0; fwd && k < count; k++) forwarding = forwarding || fwd[k].dst;
+    if (forwarding && fw.open()) return -1;
     int launches = 0;
-    g->kev_used = 0;
-    for (int k = 0; k < g->count; k++) {
-        g->m[k]->kev_used = 0;
-        if (order_enter(g->m[k], st)) return -1;
+    if (g) g->kev_used = 0;
+    for (int k = 0; k < count; k++) {
+        m[k]->kev_used = 0;
+        if (order_enter(m[k], st)) return -1;
     }
     for (int c0 = 0; c0 < nframes; c0 += CHUNK) {
-        const int nf = std::min(CHUNK, nframes - c0);
+        const int nf = std::min(CHUNK, nframes - c0), pre = c0 == 0 ? preload : 0;
         int live0[GROUP_MAX];
         short *pc[GROUP_MAX];
-        for (int k = 0; k < g->count; k++) {
-            LPCNetB200Batch *b = g->m[k];
+        for (int k = 0; k < count; k++) {
             pc[k] = pcm[k] + (size_t)c0 * spf;
-            launches += frame_chunk(b, feat[k], stream_stride, frame_stride, c0, nf, st);
-            const int r = sample_prefix(b, 0, nf, spf, pc[k], pcm_stride, 0, st, &live0[k]);
+            launches += frame_chunk(m[k], feat[k], stream_stride, c.stride, c0, nf, st);
+            const int r = sample_prefix(m[k], 0, nf, spf, pc[k], pcm_stride, pre, st, &live0[k]);
             if (r < 0) return -1;
             launches += r;
         }
-        const int r = launch_group(g, live0, nf, spf, pc, pcm_stride, st);
+        const int r = g ? launch_group(g, live0, nf, spf, pc, pcm_stride, st) : launch_rest(b, 0, live0[0], nf, spf, pc[0], pcm_stride, pre, st);
         if (r < 0) return -1;
         launches += r;
-        for (int k = 0; k < g->count; k++) for (int &v : g->m[k]->fc) v = std::min(1000, v + nf);
-        for (int k = 0; forwarding && k < g->count; k++)
-            if (fwd[k].dst && forward_chunk(fwd[k], g->m[k]->n, pcm[k], pcm_stride, c0, nf, spf, st, g->fwd_stream, g->fwd_ev)) return -1;
+        for (int k = 0; k < count; k++) for (int &v : m[k]->fc) v = std::min(1000, v + nf);
+        for (int k = 0; forwarding && k < count; k++)
+            if (fwd[k].dst && fw.forward_to_sink(fwd[k], m[k]->n, pcm[k], pcm_stride, c0, nf, spf, st)) return -1;
     }
     CK(cudaGetLastError());
-    if (forwarding) {    // the call's completion includes the forwarded PCM
-        CK(cudaEventRecord(g->fwd_done, g->fwd_stream));
-        CK(cudaStreamWaitEvent(st, g->fwd_done, 0));
-    }
-    for (int k = 0; k < g->count; k++) if (order_leave(g->m[k], st)) return -1;
-    g->last_launches = launches;
+    if (forwarding && fw.join(st)) return -1;
+    for (int k = 0; k < count; k++) if (order_leave(m[k], st)) return -1;
+    (g ? g->last_launches : b->last_launches) = launches + (c.decode ? count : 0);    // (+ the packet decoders)
+    return 0;
+}
+
+// What a public group call refuses, in this order: a NULL group, a member with a PCM sink, NULL buffers, a bad shape, a decode
+// with a member without codebooks.  Returns 1 for a call without units: nothing to do.
+static int group_entry(LPCNetB200Group *g, const CallShape &c, const void *in, const void *out)
+{
+    if (group_check(g, CallShape{}, true)) return -1;
+    CK(cudaSetDevice(g->device));
+    if (c.units <= 0) return 1;
+    if (!in || !out) { set_error("null buffer"); return -1; }
+    return group_check(g, c, false);
+}
+// a checked call on device buffers of the group's rows
+static int group_call_rows(LPCNetB200Group *g, const CallShape &c, const void *in, short *pcm, cudaStream_t st)
+{
+    const void *pin[GROUP_MAX]; short *ppcm[GROUP_MAX];
+    group_rows(g, c, in, pcm, nullptr, pin, ppcm);
+    return group_call(g, c, pin, ppcm, nullptr, st);
+}
+static int group_device(LPCNetB200Group *g, const CallShape &c, const void *d_in, short *d_pcm, void *cuda_stream)
+{
+    const int r = group_entry(g, c, d_in, d_pcm);
+    if (r) return r < 0 ? -1 : 0;
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
+    if (group_call_rows(g, c, d_in, d_pcm, st)) return -1;
+    if (!cuda_stream) CK(cudaStreamSynchronize(st));
+    return 0;
+}
+// host-pointer calls: the rows go through the group's own staging buffers on its stream; returns once the PCM is on the host
+static int group_host(LPCNetB200Group *g, const CallShape &c, const void *in, short *pcm)
+{
+    const int r = group_entry(g, c, in, pcm);
+    if (r) return r < 0 ? -1 : 0;
+    const size_t in_bytes = c.in_bytes() * g->n_total, pcm_bytes = sizeof(short) * c.pcm_samples() * g->n_total;
+    // (earlier host calls are complete and `_device` calls never touch these buffers: nothing can still be using them)
+    if (grow_buffer(&g->d_in, &g->d_in_cap, in_bytes) || grow_buffer((void **)&g->d_pcm, &g->d_pcm_cap, pcm_bytes)) return -1;
+    CK(cudaMemcpyAsync(g->d_in, in, in_bytes, cudaMemcpyHostToDevice, g->stream));
+    if (group_call_rows(g, c, g->d_in, g->d_pcm, g->stream)) return -1;
+    CK(cudaMemcpyAsync(pcm, g->d_pcm, pcm_bytes, cudaMemcpyDeviceToHost, g->stream));
+    CK(cudaStreamSynchronize(g->stream));
     return 0;
 }
 
 int lpcnet_b200_group_synthesize_device(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride,
                                         int samples_per_frame, short *d_pcm, void *cuda_stream)
 {
-    if (group_check(g)) return -1;
-    if (nframes <= 0) return 0;
-    if (!d_features || !d_pcm) { set_error("null buffer"); return -1; }
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
-    int r = group_synthesize_forward(g, d_features, nframes, feature_stride, samples_per_frame, d_pcm, nullptr, st);
-    if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
-    return r;
+    return group_device(g, CallShape::synthesis(nframes, feature_stride, samples_per_frame), d_features, d_pcm, cuda_stream);
 }
-
 int lpcnet_b200_group_synthesize(LPCNetB200Group *g, const float *features, int nframes, int feature_stride,
                                  int samples_per_frame, short *pcm)
 {
-    if (group_check(g)) return -1;
-    if (nframes <= 0) return 0;
-    if (!features || !pcm) { set_error("null buffer"); return -1; }
-    const float *feat[GROUP_MAX]; short *dp[GROUP_MAX];
-    for (int k = 0; k < g->count; k++) {      // each member's rows go through the member's own staging buffers
-        LPCNetB200Batch *b = g->m[k];
-        if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * (size_t)b->n * nframes * feature_stride)) return -1;
-        if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, sizeof(short) * (size_t)b->n * nframes * samples_per_frame)) return -1;
-        feat[k] = b->d_features; dp[k] = b->d_pcm;
-    }
-    size_t row = 0;
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        if (order_enter(b, g->stream)) return -1;
-        CK(cudaMemcpyAsync(b->d_features, features + row * nframes * feature_stride, sizeof(float) * (size_t)b->n * nframes * feature_stride,
-                           cudaMemcpyHostToDevice, g->stream));
-        if (order_leave(b, g->stream)) return -1;
-        row += b->n;
-    }
-    if (group_synth(g, feat, feature_stride, nframes, samples_per_frame, dp, nullptr, g->stream)) return -1;
-    row = 0;
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        CK(cudaMemcpyAsync(pcm + row * nframes * samples_per_frame, b->d_pcm, sizeof(short) * (size_t)b->n * nframes * samples_per_frame,
-                           cudaMemcpyDeviceToHost, g->stream));
-        row += b->n;
-    }
-    CK(cudaStreamSynchronize(g->stream));
-    return 0;
+    return group_host(g, CallShape::synthesis(nframes, feature_stride, samples_per_frame), features, pcm);
 }
-
-// decode: every member's packet decoder into the member's feature staging, then the group synthesis over those features
-static int group_decode(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, const PcmTarget *fwd, cudaStream_t st)
+int lpcnet_b200_group_decode_device(LPCNetB200Group *g, const unsigned char *d_packets, int npackets, short *d_pcm, void *cuda_stream)
 {
-    if (group_call_check(g, npackets * 4, NB_FEAT, FRAME_SIZE, true)) return -1;
-    const float *feat[GROUP_MAX];
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        if (ensure(b, (void **)&b->d_features, &b->d_features_cap, sizeof(float) * (size_t)b->n * npackets * 4 * NB_FEAT)) return -1;
-        feat[k] = b->d_features;
-    }
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        if (order_enter(b, st)) return -1;
-        launch_decode_packets(b->model, b->fs, packets[k], b->n, npackets, b->d_features, st);
-        if (order_leave(b, st)) return -1;
-    }
-    if (group_synth(g, feat, NB_FEAT, npackets * 4, FRAME_SIZE, pcm, fwd, st)) return -1;
-    g->last_launches += g->count;
-    return 0;
+    return group_device(g, CallShape::packets(npackets), d_packets, d_pcm, cuda_stream);
+}
+int lpcnet_b200_group_decode(LPCNetB200Group *g, const unsigned char *packets, int npackets, short *pcm)
+{
+    return group_host(g, CallShape::packets(npackets), packets, pcm);
 }
 
 }  // extern "C"
@@ -1168,108 +1155,33 @@ int lpcnet_b200::mixed_plan(const int *n, const int *na, const int *is_float, in
     return classes;
 }
 
-int lpcnet_b200::group_check(LPCNetB200Group *g)
+int lpcnet_b200::group_check(const LPCNetB200Group *g, const CallShape &c, bool refuse_sinks)
 {
     if (!g) { set_error("null group"); return -1; }
-    for (int k = 0; k < g->count; k++)
-        if (g->m[k]->sink) { set_error("group call: member %d has a PCM sink set; groups do not forward PCM to sinks", k); return -1; }
-    CK(cudaSetDevice(g->device));
+    for (int k = 0; refuse_sinks && k < g->count; k++)
+        if (g->m[k]->sink.dst) { set_error("group call: member %d has a PCM sink set; groups do not forward PCM to sinks", k); return -1; }
+    if (c.units <= 0) return 0;
+    if (c.check()) return -1;
+    for (int k = 0; c.decode && k < g->count; k++)
+        if (!g->m[k]->model.codebooks) { set_error("group decode: member %d has no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)", k); return -1; }
     return 0;
 }
 
-int lpcnet_b200::group_synthesize_members(LPCNetB200Group *g, const float *const *feat, int nframes, int feature_stride, int spf,
-                                          short *const *pcm, cudaStream_t st)
+void lpcnet_b200::group_rows(const LPCNetB200Group *g, const CallShape &c, const void *in, short *pcm, const int *rows, const void **pin, short **ppcm)
 {
-    return group_synth(g, feat, feature_stride, nframes, spf, pcm, nullptr, st);
-}
-
-int lpcnet_b200::group_decode_members(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, cudaStream_t st)
-{
-    return group_decode(g, packets, npackets, pcm, nullptr, st);
-}
-
-// ---- the entries of the multi-GPU groups (engine.h) ----
-int lpcnet_b200::group_call_check(const LPCNetB200Group *g, int nframes, int frame_stride, int spf, bool decode)
-{
-    if (!g) { set_error("null group"); return -1; }
-    if (nframes <= 0) return 0;
-    if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
-    if (frame_stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
-    if (decode)
-        for (int k = 0; k < g->count; k++)
-            if (!g->m[k]->model.codebooks) { set_error("group decode: member %d has no VQ codebooks loaded (lpcnet_b200_batch_set_codebooks)", k); return -1; }
-    return 0;
-}
-
-// group rows in one device buffer each: member k's features and PCM at its first row
-int lpcnet_b200::group_synthesize_forward(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride, int spf, short *d_pcm,
-                                          const PcmTarget *fwd, cudaStream_t st)
-{
-    const float *feat[GROUP_MAX] = {}; short *pcm[GROUP_MAX] = {};
-    size_t row = 0;
-    for (int k = 0; k < g->count; k++) {
-        feat[k] = d_features + row * nframes * feature_stride;
-        pcm[k] = d_pcm + row * nframes * spf;
-        row += g->m[k]->n;
+    for (int k = 0, row = 0; k < g->count; row += g->m[k]->n, k++) {
+        const size_t r = rows ? rows[k] : row;
+        pin[k] = (const char *)in + c.in_bytes() * r;
+        ppcm[k] = pcm + c.pcm_samples() * r;
     }
-    return group_synth(g, feat, feature_stride, nframes, spf, pcm, fwd, st);
 }
 
-int lpcnet_b200::group_decode_forward(LPCNetB200Group *g, const uint8_t *d_packets, int npackets, short *d_pcm, const PcmTarget *fwd, cudaStream_t st)
+int lpcnet_b200::group_call(LPCNetB200Group *g, const CallShape &c, const void *const *in, short *const *pcm, const PcmTarget *fwd, cudaStream_t st)
 {
-    const uint8_t *pk[GROUP_MAX] = {}; short *pcm[GROUP_MAX] = {};
-    size_t row = 0;
-    for (int k = 0; k < g->count; k++) {
-        pk[k] = d_packets + row * npackets * 8;
-        pcm[k] = d_pcm + row * npackets * 640;
-        row += g->m[k]->n;
-    }
-    return group_decode(g, pk, npackets, pcm, fwd, st);
+    return run_call(g, nullptr, c, in, pcm, fwd, 0, st);
 }
 
 extern "C" {
-
-int lpcnet_b200_group_decode_device(LPCNetB200Group *g, const unsigned char *d_packets, int npackets, short *d_pcm, void *cuda_stream)
-{
-    if (group_check(g)) return -1;
-    if (npackets <= 0) return 0;
-    if (!d_packets || !d_pcm) { set_error("null buffer"); return -1; }
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : g->stream;
-    int r = group_decode_forward(g, d_packets, npackets, d_pcm, nullptr, st);
-    if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
-    return r;
-}
-
-int lpcnet_b200_group_decode(LPCNetB200Group *g, const unsigned char *packets, int npackets, short *pcm)
-{
-    if (group_check(g)) return -1;
-    if (npackets <= 0) return 0;
-    if (!packets || !pcm) { set_error("null buffer"); return -1; }
-    const uint8_t *pk[GROUP_MAX]; short *dp[GROUP_MAX];
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        if (ensure(b, (void **)&b->d_packets, &b->d_packets_cap, (size_t)b->n * npackets * 8)) return -1;
-        if (ensure(b, (void **)&b->d_pcm, &b->d_pcm_cap, sizeof(short) * (size_t)b->n * npackets * 640)) return -1;
-        pk[k] = b->d_packets; dp[k] = b->d_pcm;
-    }
-    size_t row = 0;
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        if (order_enter(b, g->stream)) return -1;
-        CK(cudaMemcpyAsync(b->d_packets, packets + row * npackets * 8, (size_t)b->n * npackets * 8, cudaMemcpyHostToDevice, g->stream));
-        if (order_leave(b, g->stream)) return -1;
-        row += b->n;
-    }
-    if (group_decode(g, pk, npackets, dp, nullptr, g->stream)) return -1;
-    row = 0;
-    for (int k = 0; k < g->count; k++) {
-        LPCNetB200Batch *b = g->m[k];
-        CK(cudaMemcpyAsync(pcm + row * npackets * 640, b->d_pcm, sizeof(short) * (size_t)b->n * npackets * 640, cudaMemcpyDeviceToHost, g->stream));
-        row += b->n;
-    }
-    CK(cudaStreamSynchronize(g->stream));
-    return 0;
-}
 
 // the group's fused launches plus the members' own launches for their silent-frame prefixes, in the last group call (the
 // latter until the member's next call)
@@ -1292,13 +1204,8 @@ int lpcnet_b200_batch_set_pcm_sink(LPCNetB200Batch *b, short *sink, long long pi
     if (!b) { set_error("null batch"); return -1; }
     CK(cudaSetDevice(b->device));
     if (order_sync(b)) return -1;
-    if (sink && !b->sink_stream) {
-        CK(cudaStreamCreateWithFlags(&b->sink_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&b->sink_ev, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&b->sink_done, cudaEventDisableTiming));
-    }
-    if (b->sink_stream) CK(cudaStreamSynchronize(b->sink_stream));
-    b->sink = sink; b->sink_pitch = pitch_samples; b->sink_row0 = first_row;
+    if (b->fwd.stream) CK(cudaStreamSynchronize(b->fwd.stream));
+    b->sink = PcmTarget{sink, pitch_samples, first_row};
     return 0;
 }
 int lpcnet_b200_ipc_export(void *d_ptr, unsigned char handle[64])

@@ -402,29 +402,34 @@ LPCNET_DECLARE_LAUNCHERS(na128)
 LPCNET_DECLARE_LAUNCHERS(na256)
 LPCNET_DECLARE_LAUNCHERS(na384)
 int sample_kernel_smem_ok(uint32_t bytes);
-int streams_per_cta_for(int n_streams, int override_spc);   // min(32, ceil(n / SM count)) on the current device unless overridden
+// grow a device buffer to at least `bytes` (the old contents are lost; nothing may still be using it); 0 / -1 (sets error)
+int grow_buffer(void **p, size_t *cap, size_t bytes);
+
+// The shape of one synthesize or decode call.  Synthesis: `units` frames of `stride` floats per stream, `spf` samples each.
+// Decode: `units` packets of 8 bytes per stream, each 4 frames of NB_FEAT features and FRAME_SIZE samples (stride, spf as such).
+struct CallShape {
+    bool decode; int units, stride, spf;
+    static CallShape synthesis(int nframes, int stride, int spf) { return CallShape{false, nframes, stride, spf}; }
+    static CallShape packets(int npackets) { return CallShape{true, npackets, NB_FEAT, FRAME_SIZE}; }
+    int frames() const { return decode ? 4 * units : units; }
+    size_t in_bytes() const { return decode ? (size_t)units * 8 : sizeof(float) * (size_t)units * stride; }      // per stream
+    long long pcm_samples() const { return (long long)frames() * spf; }                                         // per stream
+    int check() const
+    {
+        if (spf < 1 || spf > 65536) { set_error("samples_per_frame must be in 1..65536"); return -1; }
+        if (stride < NB_FEAT) { set_error("feature_stride must be >= 20"); return -1; }
+        return 0;
+    }
+};
 
 }  // namespace lpcnet_b200
 
-// ---- group calls with per-member PCM forwarding (batch_api.cu; used by the multi-GPU groups of multi_api.cu) ----
+// ---- the parts of groups that mixed groups (mixed_api.cu) and multi-GPU groups (multi_api.cu) are built from (batch_api.cu) ----
+struct LPCNetB200Batch;
 struct LPCNetB200Group;
 namespace lpcnet_b200 {
 // Where a member's PCM goes as well: after every chunk, rows s of the member's PCM land at dst[(row0 + s) * pitch + t] (dst NULL: nowhere)
 struct PcmTarget { short *dst; long long pitch, row0; };
-// Refuses (sets the error, returns -1) what a group synthesize call of nframes frames would refuse (decode: a decode call of
-// nframes / 4 packets, frame_stride 20, spf 160), without enqueueing anything.
-int group_call_check(const LPCNetB200Group *g, int nframes, int frame_stride, int spf, bool decode);
-// The group's synthesize / decode `_device` calls with fwd[k] as member k's target (fwd NULL: none).  Members' PCM sinks are
-// neither used nor refused.  Everything is enqueued on `st` (of the group's device, current); the forwarded copies are part of
-// the call's completion on `st`.
-int group_synthesize_forward(LPCNetB200Group *g, const float *d_features, int nframes, int feature_stride, int spf, short *d_pcm,
-                             const PcmTarget *fwd, cudaStream_t st);
-int group_decode_forward(LPCNetB200Group *g, const uint8_t *d_packets, int npackets, short *d_pcm, const PcmTarget *fwd, cudaStream_t st);
-}  // namespace lpcnet_b200
-
-// ---- the parts of groups that mixed groups (mixed_api.cu) are built from (batch_api.cu) ----
-struct LPCNetB200Batch;
-namespace lpcnet_b200 {
 // 1..GROUP_MAX batches, none NULL, none listed twice, all on one device; with one_shape also one GRU_A size and one flavour.
 // Otherwise sets the error (prefixed with `who`) and returns -1.
 int group_members_check(LPCNetB200Batch *const *batches, int count, const char *who, bool one_shape);
@@ -438,11 +443,15 @@ int batch_device(const LPCNetB200Batch *b);
 // Returns the number of classes.
 int mixed_plan(const int *n, const int *na, const int *is_float, int count, int sms, int override_spc, bool lane_stream,
                int *spc, int *class_of, int *class_ctas, bool *class_neuron);
-// What a public group call refuses before its arguments: a member with a PCM sink (also sets the group's device)
-int group_check(LPCNetB200Group *g);
-// The group's synthesize / decode `_device` calls with member k's inputs at feat[k] / packets[k] and its PCM at pcm[k]
-// ([n_k][nframes*spf] resp. [n_k][npackets*640]), everything on `st`; no sink check (group_check) and no forwarding.
-int group_synthesize_members(LPCNetB200Group *g, const float *const *feat, int nframes, int feature_stride, int spf,
-                             short *const *pcm, cudaStream_t st);
-int group_decode_members(LPCNetB200Group *g, const uint8_t *const *packets, int npackets, short *const *pcm, cudaStream_t st);
+// Refuses (sets the error, returns -1), without enqueueing anything: a NULL group; with refuse_sinks a member with a PCM sink
+// (public groups and mixed groups do not forward to sinks); then, for a call with units, a bad shape and a decode with a member
+// that has no codebooks.
+int group_check(const LPCNetB200Group *g, const CallShape &c, bool refuse_sinks);
+// Member k's inputs and PCM in device buffers of rows: at row rows[k] (rows NULL: the group's own layout, member 0's rows first,
+// then member 1's ...)
+void group_rows(const LPCNetB200Group *g, const CallShape &c, const void *in, short *pcm, const int *rows, const void **pin, short **ppcm);
+// A checked group call: member k's features or packets at in[k], its PCM at pcm[k] ([n_k][c.pcm_samples()]), and each chunk of
+// it forwarded to fwd[k] (fwd NULL: nowhere).  Members' own PCM sinks are not used.  Everything is enqueued on `st` (of the
+// group's device, current); the forwarded copies are part of the call's completion on `st`.
+int group_call(LPCNetB200Group *g, const CallShape &c, const void *const *in, short *const *pcm, const PcmTarget *fwd, cudaStream_t st);
 }  // namespace lpcnet_b200

@@ -27,16 +27,6 @@ struct LPCNetB200MixedGroup {
     short *d_pcm; size_t d_pcm_cap;
 };
 
-static int grow(void **p, size_t *cap, size_t bytes)
-{
-    if (*cap >= bytes) return 0;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    CK(cudaMalloc(p, bytes));
-    *cap = bytes;
-    return 0;
-}
-
 extern "C" {
 
 void lpcnet_b200_mixed_group_destroy(LPCNetB200MixedGroup *mg)
@@ -101,62 +91,64 @@ LPCNetB200Group *lpcnet_b200_mixed_group_group(LPCNetB200MixedGroup *mg, int c)
 
 }  // extern "C"
 
-// What every call refuses first, as a group call does: a member with a PCM sink
-static int mx_sinks(LPCNetB200MixedGroup *mg)
+// What a call refuses, in the order of a group call: a member with a PCM sink, NULL buffers, then what any class's group call of
+// shape c would refuse.  Returns 1 for a call without units: nothing to do.
+static int mx_check(LPCNetB200MixedGroup *mg, const CallShape &c, const void *in, const void *out)
 {
     if (!mg) { set_error("null mixed group"); return -1; }
-    for (int c = 0; c < mg->classes; c++) if (group_check(mg->g[c])) return -1;
-    return 0;
-}
-// ... and what a call of `units` frames (decode: packets) would refuse in any class's group call
-static int mx_check(LPCNetB200MixedGroup *mg, int units, int stride, int spf, bool decode)
-{
-    for (int c = 0; c < mg->classes; c++)
-        if (group_call_check(mg->g[c], decode ? units * 4 : units, decode ? NB_FEAT : stride, spf, decode)) return -1;
+    for (int k = 0; k < mg->classes; k++) if (group_check(mg->g[k], CallShape{}, true)) return -1;
+    CK(cudaSetDevice(mg->device));
+    if (c.units <= 0) return 1;
+    if (!in || !out) { set_error("null buffer"); return -1; }
+    for (int k = 0; k < mg->classes; k++) if (group_check(mg->g[k], c, false)) return -1;
     return 0;
 }
 
-// One call on device buffers `in` (features [sum n][units][stride] or packets [sum n][units][8]) and `d_pcm`, its completion on `st`:
-// class 0 on st, class c > 0 on stream[c] after the fork, every class stream joined back into st (also after an error, so that
-// nothing the call enqueued outlives it on st)
-static int mx_run(LPCNetB200MixedGroup *mg, const void *in, int units, int stride, int spf, bool decode, short *d_pcm, cudaStream_t st)
+// One checked call on device buffers `in` (features or packets, [sum n] rows) and `d_pcm`, its completion on `st`: class 0 on st,
+// class k > 0 on stream[k] after the fork, every class stream joined back into st (also after an error, so that nothing the call
+// enqueued outlives it on st)
+static int mx_run(LPCNetB200MixedGroup *mg, const CallShape &c, const void *in, short *d_pcm, cudaStream_t st)
 {
-    const size_t in_row = decode ? (size_t)units * 8 : sizeof(float) * (size_t)units * stride;
-    const size_t pcm_row = decode ? (size_t)units * 640 : (size_t)units * spf;
-    CK(cudaSetDevice(mg->device));
     CK(cudaEventRecord(mg->fork, st));
     int rc = 0, started = 0;
-    for (int c = 0; c < mg->classes && rc == 0; c++) {
-        cudaStream_t cs = c ? mg->stream[c] : st;
-        if (c && cudaStreamWaitEvent(cs, mg->fork, 0) != cudaSuccess) { set_error("mixed_group: fork failed"); rc = -1; break; }
+    for (int k = 0; k < mg->classes && rc == 0; k++) {
+        cudaStream_t cs = k ? mg->stream[k] : st;
+        if (k && cudaStreamWaitEvent(cs, mg->fork, 0) != cudaSuccess) { set_error("mixed_group: fork failed"); rc = -1; break; }
         started++;
         const void *pin[GROUP_MAX]; short *pcm[GROUP_MAX];
-        for (int j = 0; j < mg->members[c]; j++) {
-            pin[j] = (const char *)in + in_row * mg->rows[c][j];
-            pcm[j] = d_pcm + pcm_row * mg->rows[c][j];
-        }
-        rc = decode ? group_decode_members(mg->g[c], (const uint8_t *const *)pin, units, pcm, cs)
-                    : group_synthesize_members(mg->g[c], (const float *const *)pin, units, stride, spf, pcm, cs);
+        group_rows(mg->g[k], c, in, d_pcm, mg->rows[k], pin, pcm);
+        rc = group_call(mg->g[k], c, pin, pcm, nullptr, cs);
     }
-    for (int c = 1; c < started; c++) {
-        CK(cudaEventRecord(mg->join[c], mg->stream[c]));
-        CK(cudaStreamWaitEvent(st, mg->join[c], 0));
+    for (int k = 1; k < started; k++) {
+        CK(cudaEventRecord(mg->join[k], mg->stream[k]));
+        CK(cudaStreamWaitEvent(st, mg->join[k], 0));
     }
     CK(cudaEventRecord(mg->done, st));
     mg->timed = true;
     return rc;
 }
 
-// host-pointer calls: the rows go through the mixed group's own staging buffers on stream[0]; returns once the PCM is on the host
-static int mx_host(LPCNetB200MixedGroup *mg, const void *in, int units, int stride, int spf, bool decode, short *pcm)
+static int mx_device(LPCNetB200MixedGroup *mg, const CallShape &c, const void *d_in, short *d_pcm, void *cuda_stream)
 {
-    const size_t in_bytes = (decode ? (size_t)units * 8 : sizeof(float) * (size_t)units * stride) * mg->n_total;
-    const size_t pcm_bytes = sizeof(short) * (decode ? (size_t)units * 640 : (size_t)units * spf) * mg->n_total;
+    const int r = mx_check(mg, c, d_in, d_pcm);
+    if (r) return r < 0 ? -1 : 0;
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : mg->stream[0];
+    if (mx_run(mg, c, d_in, d_pcm, st)) return -1;
+    if (!cuda_stream) CK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// host-pointer calls: the rows go through the mixed group's own staging buffers on stream[0]; returns once the PCM is on the host
+static int mx_host(LPCNetB200MixedGroup *mg, const CallShape &c, const void *in, short *pcm)
+{
+    const int r = mx_check(mg, c, in, pcm);
+    if (r) return r < 0 ? -1 : 0;
+    const size_t in_bytes = c.in_bytes() * mg->n_total, pcm_bytes = sizeof(short) * c.pcm_samples() * mg->n_total;
     cudaStream_t st = mg->stream[0];
     // (earlier host calls are complete and `_device` calls never touch these buffers: nothing can still be using them)
-    if (grow(&mg->d_in, &mg->d_in_cap, in_bytes) || grow((void **)&mg->d_pcm, &mg->d_pcm_cap, pcm_bytes)) return -1;
+    if (grow_buffer(&mg->d_in, &mg->d_in_cap, in_bytes) || grow_buffer((void **)&mg->d_pcm, &mg->d_pcm_cap, pcm_bytes)) return -1;
     CK(cudaMemcpyAsync(mg->d_in, in, in_bytes, cudaMemcpyHostToDevice, st));
-    int rc = mx_run(mg, mg->d_in, units, stride, spf, decode, mg->d_pcm, st);
+    int rc = mx_run(mg, c, mg->d_in, mg->d_pcm, st);
     if (rc == 0) CK(cudaMemcpyAsync(pcm, mg->d_pcm, pcm_bytes, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return rc;
@@ -167,46 +159,24 @@ extern "C" {
 int lpcnet_b200_mixed_group_synthesize(LPCNetB200MixedGroup *mg, const float *features, int nframes, int feature_stride,
                                        int samples_per_frame, short *pcm)
 {
-    if (mx_sinks(mg)) return -1;
-    if (nframes <= 0) return 0;
-    if (!features || !pcm) { set_error("null buffer"); return -1; }
-    if (mx_check(mg, nframes, feature_stride, samples_per_frame, false)) return -1;
-    return mx_host(mg, features, nframes, feature_stride, samples_per_frame, false, pcm);
+    return mx_host(mg, CallShape::synthesis(nframes, feature_stride, samples_per_frame), features, pcm);
 }
 
 int lpcnet_b200_mixed_group_synthesize_device(LPCNetB200MixedGroup *mg, const float *d_features, int nframes, int feature_stride,
                                               int samples_per_frame, short *d_pcm, void *cuda_stream)
 {
-    if (mx_sinks(mg)) return -1;
-    if (nframes <= 0) return 0;
-    if (!d_features || !d_pcm) { set_error("null buffer"); return -1; }
-    if (mx_check(mg, nframes, feature_stride, samples_per_frame, false)) return -1;
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : mg->stream[0];
-    int r = mx_run(mg, d_features, nframes, feature_stride, samples_per_frame, false, d_pcm, st);
-    if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
-    return r;
+    return mx_device(mg, CallShape::synthesis(nframes, feature_stride, samples_per_frame), d_features, d_pcm, cuda_stream);
 }
 
 int lpcnet_b200_mixed_group_decode(LPCNetB200MixedGroup *mg, const unsigned char *packets, int npackets, short *pcm)
 {
-    if (mx_sinks(mg)) return -1;
-    if (npackets <= 0) return 0;
-    if (!packets || !pcm) { set_error("null buffer"); return -1; }
-    if (mx_check(mg, npackets, NB_FEAT, FRAME_SIZE, true)) return -1;
-    return mx_host(mg, packets, npackets, NB_FEAT, FRAME_SIZE, true, pcm);
+    return mx_host(mg, CallShape::packets(npackets), packets, pcm);
 }
 
 int lpcnet_b200_mixed_group_decode_device(LPCNetB200MixedGroup *mg, const unsigned char *d_packets, int npackets, short *d_pcm,
                                           void *cuda_stream)
 {
-    if (mx_sinks(mg)) return -1;
-    if (npackets <= 0) return 0;
-    if (!d_packets || !d_pcm) { set_error("null buffer"); return -1; }
-    if (mx_check(mg, npackets, NB_FEAT, FRAME_SIZE, true)) return -1;
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : mg->stream[0];
-    int r = mx_run(mg, d_packets, npackets, NB_FEAT, FRAME_SIZE, true, d_pcm, st);
-    if (r == 0 && !cuda_stream) CK(cudaStreamSynchronize(st));
-    return r;
+    return mx_device(mg, CallShape::packets(npackets), d_packets, d_pcm, cuda_stream);
 }
 
 float lpcnet_b200_mixed_group_last_call_ms(const LPCNetB200MixedGroup *mg)

@@ -12,7 +12,7 @@
 // One process per GPU (torchrun / MPI style) uses the same sink through CUDA IPC instead: lpcnet_b200_ipc_export/_open.
 // Multi-GPU groups (lpcnet_b200_multi_group_*) serve several models, one LPCNetB200Multi each over the same devices, the same way:
 // per device one group over the members' shards, and the gather forwarded from inside the group's chunk loop
-// (batch_api.cu group_synthesize_forward) instead of through the shard batches' sinks.
+// (batch_api.cu group_call with forward targets) instead of through the shard batches' sinks.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -37,16 +37,6 @@ struct LPCNetB200Multi {
     std::vector<Shard> shards;
     bool peer_ok;                         // every device can write the memory of devices[0]
 };
-
-static int grow(void **p, size_t *cap, size_t bytes)
-{
-    if (*cap >= bytes) return 0;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *cap = 0;
-    CK(cudaMalloc(p, bytes));
-    *cap = bytes;
-    return 0;
-}
 
 extern "C" {
 
@@ -147,21 +137,20 @@ int lpcnet_b200_multi_set_codebooks(LPCNetB200Multi *m, const float *cb, size_t 
 
 // Shared body.  in: host features [n][nframes][stride] (packets: [n][npackets][8]); out: host pcm [n][T] (gather_dev == NULL)
 // or the gather buffer d_gather [n][T] in the memory of devices[0].
-static int run_all(LPCNetB200Multi *m, const void *in, size_t in_row_bytes, int units, int stride, int spf, bool decode,
-                   short *pcm_host, short *d_gather)
+static int run_all(LPCNetB200Multi *m, const CallShape &c, const void *in, short *pcm_host, short *d_gather)
 {
-    const long long T = decode ? (long long)units * 640 : (long long)units * spf;
+    const long long T = c.pcm_samples();
     int rc = 0;
     // enqueue everything on every device first ...
     for (Shard &s : m->shards) {
         CK(cudaSetDevice(s.device));
-        const size_t ibytes = in_row_bytes * s.count, pbytes = sizeof(short) * (size_t)T * s.count;
+        const size_t ibytes = c.in_bytes() * s.count, pbytes = sizeof(short) * (size_t)T * s.count;
         CK(cudaStreamSynchronize(s.stream));                                   // previous call's users of the staging buffers
-        if (grow(&s.d_in, &s.d_in_cap, ibytes) || grow((void **)&s.d_pcm, &s.d_pcm_cap, pbytes)) return -1;
+        if (grow_buffer(&s.d_in, &s.d_in_cap, ibytes) || grow_buffer((void **)&s.d_pcm, &s.d_pcm_cap, pbytes)) return -1;
         if (lpcnet_b200_batch_set_pcm_sink(s.batch, d_gather, T, s.first)) return -1;   // NULL removes it
-        CK(cudaMemcpyAsync(s.d_in, (const char *)in + in_row_bytes * s.first, ibytes, cudaMemcpyHostToDevice, s.stream));
-        const int r = decode ? lpcnet_b200_batch_decode_device(s.batch, (const unsigned char *)s.d_in, units, s.d_pcm, s.stream)
-                             : lpcnet_b200_batch_synthesize_device(s.batch, (const float *)s.d_in, units, stride, spf, s.d_pcm, s.stream);
+        CK(cudaMemcpyAsync(s.d_in, (const char *)in + c.in_bytes() * s.first, ibytes, cudaMemcpyHostToDevice, s.stream));
+        const int r = c.decode ? lpcnet_b200_batch_decode_device(s.batch, (const unsigned char *)s.d_in, c.units, s.d_pcm, s.stream)
+                               : lpcnet_b200_batch_synthesize_device(s.batch, (const float *)s.d_in, c.units, c.stride, c.spf, s.d_pcm, s.stream);
         if (r) { rc = -1; break; }
         if (pcm_host) CK(cudaMemcpyAsync(pcm_host + (size_t)T * s.first, s.d_pcm, pbytes, cudaMemcpyDeviceToHost, s.stream));
     }
@@ -177,25 +166,25 @@ int lpcnet_b200_multi_synthesize(LPCNetB200Multi *m, const float *features, int 
 {
     if (!m || !features || !pcm) { set_error("multi_synthesize: null argument"); return -1; }
     if (nframes <= 0) return 0;
-    return run_all(m, features, sizeof(float) * (size_t)nframes * feature_stride, nframes, feature_stride, samples_per_frame, false, pcm, nullptr);
+    return run_all(m, CallShape::synthesis(nframes, feature_stride, samples_per_frame), features, pcm, nullptr);
 }
 int lpcnet_b200_multi_synthesize_gather(LPCNetB200Multi *m, const float *features, int nframes, int feature_stride, int samples_per_frame, short *d_pcm)
 {
     if (!m || !features || !d_pcm) { set_error("multi_synthesize_gather: null argument"); return -1; }
     if (nframes <= 0) return 0;
-    return run_all(m, features, sizeof(float) * (size_t)nframes * feature_stride, nframes, feature_stride, samples_per_frame, false, nullptr, d_pcm);
+    return run_all(m, CallShape::synthesis(nframes, feature_stride, samples_per_frame), features, nullptr, d_pcm);
 }
 int lpcnet_b200_multi_decode(LPCNetB200Multi *m, const unsigned char *packets, int npackets, short *pcm)
 {
     if (!m || !packets || !pcm) { set_error("multi_decode: null argument"); return -1; }
     if (npackets <= 0) return 0;
-    return run_all(m, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, pcm, nullptr);
+    return run_all(m, CallShape::packets(npackets), packets, pcm, nullptr);
 }
 int lpcnet_b200_multi_decode_gather(LPCNetB200Multi *m, const unsigned char *packets, int npackets, short *d_pcm)
 {
     if (!m || !packets || !d_pcm) { set_error("multi_decode_gather: null argument"); return -1; }
     if (npackets <= 0) return 0;
-    return run_all(m, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, nullptr, d_pcm);
+    return run_all(m, CallShape::packets(npackets), packets, nullptr, d_pcm);
 }
 
 // ---- multi-GPU groups: several models, each an LPCNetB200Multi over the same devices, in one call ----
@@ -283,25 +272,26 @@ LPCNetB200Group *lpcnet_b200_multi_group_group(LPCNetB200MultiGroup *mg, int k)
     return mg->dev[k].group;
 }
 
-// One device's share of a call, enqueued on its stream: every member's rows up, then the group call, which forwards each chunk to
-// the gather buffer if there is one
-static int mg_enqueue(LPCNetB200MultiGroup *mg, size_t k, const void *in, size_t in_row_bytes, int units, int stride, int spf, bool decode,
-                      long long T, short *d_gather)
+// One device's share of a checked call, enqueued on its stream: every member's rows up, then the group call, which forwards each
+// chunk to the gather buffer if there is one
+static int mg_enqueue(LPCNetB200MultiGroup *mg, size_t k, const CallShape &c, const void *in, short *d_gather)
 {
     MGDevice &d = mg->dev[k];
+    const long long T = c.pcm_samples();
     CK(cudaSetDevice(d.device));
-    if (grow(&d.d_in, &d.d_in_cap, in_row_bytes * d.rows) || grow((void **)&d.d_pcm, &d.d_pcm_cap, sizeof(short) * (size_t)T * d.rows)) return -1;
+    if (grow_buffer(&d.d_in, &d.d_in_cap, c.in_bytes() * d.rows) || grow_buffer((void **)&d.d_pcm, &d.d_pcm_cap, sizeof(short) * (size_t)T * d.rows)) return -1;
     PcmTarget fwd[GROUP_MAX];
     int local = 0;
     for (size_t j = 0; j < mg->m.size(); j++) {
         const Shard &s = mg->m[j]->shards[k];
         const long long row = mg->base[j] + s.first;
         fwd[j] = PcmTarget{d_gather, T, row};
-        CK(cudaMemcpyAsync((char *)d.d_in + in_row_bytes * local, (const char *)in + in_row_bytes * row, in_row_bytes * s.count, cudaMemcpyHostToDevice, d.stream));
+        CK(cudaMemcpyAsync((char *)d.d_in + c.in_bytes() * local, (const char *)in + c.in_bytes() * row, c.in_bytes() * s.count, cudaMemcpyHostToDevice, d.stream));
         local += s.count;
     }
-    return decode ? group_decode_forward(d.group, (const uint8_t *)d.d_in, units, d.d_pcm, d_gather ? fwd : nullptr, d.stream)
-                  : group_synthesize_forward(d.group, (const float *)d.d_in, units, stride, spf, d.d_pcm, d_gather ? fwd : nullptr, d.stream);
+    const void *pin[GROUP_MAX]; short *pcm[GROUP_MAX];
+    group_rows(d.group, c, d.d_in, d.d_pcm, nullptr, pin, pcm);
+    return group_call(d.group, c, pin, pcm, d_gather ? fwd : nullptr, d.stream);
 }
 // ... and its rows of every member down to the host
 static int mg_download(LPCNetB200MultiGroup *mg, size_t k, long long T, short *pcm_host)
@@ -318,17 +308,15 @@ static int mg_download(LPCNetB200MultiGroup *mg, size_t k, long long T, short *p
     return 0;
 }
 
-static int mg_run(LPCNetB200MultiGroup *mg, const void *in, size_t in_row_bytes, int units, int stride, int spf, bool decode,
-                  short *pcm_host, short *d_gather)
+static int mg_run(LPCNetB200MultiGroup *mg, const CallShape &c, const void *in, short *pcm_host, short *d_gather)
 {
     for (MGDevice &d : mg->dev)          // refuse before anything is enqueued on any device
-        if (group_call_check(d.group, decode ? units * 4 : units, decode ? NB_FEAT : stride, spf, decode)) return -1;
-    const long long T = decode ? (long long)units * 640 : (long long)units * spf;
+        if (group_check(d.group, c, false)) return -1;
     int rc = 0;
     // enqueue the work of every device first, the copies to the host after it (a copy to pageable memory returns only once it
     // is done: it must not hold back the next device's work) ...
-    for (size_t k = 0; k < mg->dev.size() && rc == 0; k++) rc = mg_enqueue(mg, k, in, in_row_bytes, units, stride, spf, decode, T, d_gather);
-    for (size_t k = 0; pcm_host && k < mg->dev.size() && rc == 0; k++) rc = mg_download(mg, k, T, pcm_host);
+    for (size_t k = 0; k < mg->dev.size() && rc == 0; k++) rc = mg_enqueue(mg, k, c, in, d_gather);
+    for (size_t k = 0; pcm_host && k < mg->dev.size() && rc == 0; k++) rc = mg_download(mg, k, c.pcm_samples(), pcm_host);
     // ... then wait for all of them (also on the error path: nothing may still be reading the caller's buffers)
     for (MGDevice &d : mg->dev) {
         cudaSetDevice(d.device);
@@ -341,25 +329,25 @@ int lpcnet_b200_multi_group_synthesize(LPCNetB200MultiGroup *mg, const float *fe
 {
     if (!mg || !features || !pcm) { set_error("multi_group_synthesize: null argument"); return -1; }
     if (nframes <= 0) return 0;
-    return mg_run(mg, features, sizeof(float) * (size_t)nframes * feature_stride, nframes, feature_stride, samples_per_frame, false, pcm, nullptr);
+    return mg_run(mg, CallShape::synthesis(nframes, feature_stride, samples_per_frame), features, pcm, nullptr);
 }
 int lpcnet_b200_multi_group_synthesize_gather(LPCNetB200MultiGroup *mg, const float *features, int nframes, int feature_stride, int samples_per_frame, short *d_pcm)
 {
     if (!mg || !features || !d_pcm) { set_error("multi_group_synthesize_gather: null argument"); return -1; }
     if (nframes <= 0) return 0;
-    return mg_run(mg, features, sizeof(float) * (size_t)nframes * feature_stride, nframes, feature_stride, samples_per_frame, false, nullptr, d_pcm);
+    return mg_run(mg, CallShape::synthesis(nframes, feature_stride, samples_per_frame), features, nullptr, d_pcm);
 }
 int lpcnet_b200_multi_group_decode(LPCNetB200MultiGroup *mg, const unsigned char *packets, int npackets, short *pcm)
 {
     if (!mg || !packets || !pcm) { set_error("multi_group_decode: null argument"); return -1; }
     if (npackets <= 0) return 0;
-    return mg_run(mg, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, pcm, nullptr);
+    return mg_run(mg, CallShape::packets(npackets), packets, pcm, nullptr);
 }
 int lpcnet_b200_multi_group_decode_gather(LPCNetB200MultiGroup *mg, const unsigned char *packets, int npackets, short *d_pcm)
 {
     if (!mg || !packets || !d_pcm) { set_error("multi_group_decode_gather: null argument"); return -1; }
     if (npackets <= 0) return 0;
-    return mg_run(mg, packets, (size_t)npackets * 8, npackets, 0, FRAME_SIZE, true, nullptr, d_pcm);
+    return mg_run(mg, CallShape::packets(npackets), packets, nullptr, d_pcm);
 }
 
 // memory on a given device (the gather buffer lives on devices[0])

@@ -1,6 +1,6 @@
 """GPU tests (-m gpu) of launch geometry: the per-sample kernels at every streams-per-CTA value (spc), at the batch sizes where the
 automatic schedule switches kernel or schedule, past one wave of CTAs, and the one-device multi API at the width of a 32768-stream
-job.  The launcher (batch_api.cu streams_per_cta_for / launch_sample) turns n streams into spc = ceil(n / SMs), clamped to 1..32,
+job.  The launcher (batch_api.cu group_plan / launch_sample) turns n streams into spc = ceil(n / SMs), clamped to 1..32,
 and picks from it:
   * int8: one half (spc <= 16) or two halves (17..32; half A takes ceil(spc / 2) slots);
   * float: the neuron-per-lane kernel (spc <= 4: its 1-, 2- or 4-slot instance) or the lane==stream kernel (5..32);

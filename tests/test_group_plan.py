@@ -94,7 +94,7 @@ def test_override_is_honoured(L, sizes, override):
 @pytest.mark.parametrize("sms", [132, 133])
 @pytest.mark.parametrize("n", [1, 2, 131, 132, 133, 263, 264, 265, 1024, 4095, 4096, 4224, 4225, 4257, 40000])
 def test_one_member_plans_like_a_batch(L, n, sms):
-    # streams_per_cta_for (batch_api.cu): min(32, max(1, ceil(n / SMs)))
+    # a batch's plan (launch_sample, batch_api.cu) in closed form: min(32, max(1, ceil(n / SMs)))
     spc, ctas = api.group_plan([n], sms)
     assert spc == min(SPC_MAX, max(1, math.ceil(n / sms)))
     assert ctas == math.ceil(n / spc)

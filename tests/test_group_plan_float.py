@@ -73,7 +73,7 @@ def test_every_stream_in_one_live_slot_and_no_cta_mixes_members(L, sizes, sms, l
 @pytest.mark.parametrize("sms", [132, 133])
 @pytest.mark.parametrize("n", [1, 2, 131, 132, 133, 263, 264, 265, 395, 396, 397, 527, 528, 529, 1024, 4224, 4225, 40000])
 def test_one_member_plans_like_a_batch(L, n, sms, override, lane_stream):
-    # streams_per_cta_for (batch_api.cu): min(32, max(1, override or ceil(n / SMs))); then the small_float rule of launch_sample
+    # a batch's plan (launch_sample, batch_api.cu) in closed form: min(32, max(1, override or ceil(n / SMs))); then its float kernel
     spc = min(SPC_MAX, max(1, override or math.ceil(n / sms)))
     small_float = spc <= FN_S and not lane_stream
     S = (1 if spc <= 1 else 2 if spc == 2 else FN_S) if small_float else spc
