@@ -78,7 +78,7 @@ LPCNET_EXPORT int lpcnet_b200_version(void);
  * blob (same format/validation as reference lpcnet_load_model, src/lpcnet.c:202 + src/parse_lpcnet_weights.c:115-221;
  * both the int8 DOT_PROD and the float flavour are accepted and select the arithmetic).  `lpc_gamma` is the
  * reference's compile-time LPC_GAMMA (generated nnet_data.h; training_tf2/dump_lpcnet.py:313-319); pass 1.0f for
- * "no weighting".  Returns NULL on error. */
+ * "no weighting", or 0 to take it from the blob's metadata record (1 without one).  Returns NULL on error. */
 LPCNET_EXPORT LPCNetB200Batch *lpcnet_b200_batch_create(int n_streams, const unsigned char *blob, int blob_len,
                                                         float lpc_gamma, int device);
 /* Same with the per-model switches given explicitly (NULL: blob metadata / defaults).  The number of GRU_A units is read

@@ -449,14 +449,16 @@ class EncBatch:
 class Batch:
     """n independent synthesis streams stepped in lockstep on one GPU (include/lpcnet_b200.h)."""
 
-    def __init__(self, n_streams, blob, lpc_gamma=1.0, device=0, codebooks=None, config=None):
-        """config: (lpc_gamma, features_delay, end2end) -> lpcnet_b200_batch_create_ex; None -> lpcnet_b200_batch_create(lpc_gamma)."""
+    def __init__(self, n_streams, blob, lpc_gamma=None, device=0, codebooks=None, config=None):
+        """config: (lpc_gamma, features_delay, end2end) -> lpcnet_b200_batch_create_ex; None -> lpcnet_b200_batch_create(lpc_gamma).
+        lpc_gamma None: the blob's metadata record supplies it (tools/import_nnet_data.py embeds nnet_data.h's LPC_GAMMA), else 1."""
         self._L = lib()
         if config is not None:
             c = Config(float(config[0]), int(config[1]), int(config[2]))
             self._h = self._L.lpcnet_b200_batch_create_ex(int(n_streams), blob, len(blob), ctypes.byref(c), int(device))
         else:
-            self._h = self._L.lpcnet_b200_batch_create(int(n_streams), blob, len(blob), float(lpc_gamma), int(device))
+            self._h = self._L.lpcnet_b200_batch_create(int(n_streams), blob, len(blob),
+                                                        0.0 if lpc_gamma is None else float(lpc_gamma), int(device))
         if not self._h:
             raise LPCNetB200Error("lpcnet_b200_batch_create: " + _err())
         self.n = int(n_streams)

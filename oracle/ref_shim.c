@@ -52,13 +52,14 @@ int ref_is_float_build(void)
 #endif
 }
 
-/* Synthesise nframes frames (features: [nframes][stride] floats, first 20 used) with a fresh state. */
+/* Synthesise nframes frames (features: [nframes][stride] floats, first 20 used) with a fresh state.  blob NULL: keep the
+ * model lpcnet_create() set up, i.e. the arrays compiled in from nnet_data.c (a build without USE_WEIGHTS_FILE). */
 int ref_synth_stream(const unsigned char *blob, int len, const float *features, int stride, int nframes,
                      short *pcm)
 {
     int i;
     LPCNetState *st = lpcnet_create();
-    if (lpcnet_load_model(st, blob, len) != 0) { lpcnet_destroy(st); return -1; }
+    if (blob && lpcnet_load_model(st, blob, len) != 0) { lpcnet_destroy(st); return -1; }
     for (i = 0; i < nframes; i++)
         lpcnet_synthesize(st, features + (size_t)i * stride, pcm + (size_t)i * LPCNET_FRAME_SIZE, LPCNET_FRAME_SIZE);
     lpcnet_destroy(st);
@@ -66,12 +67,12 @@ int ref_synth_stream(const unsigned char *blob, int len, const float *features, 
 }
 
 /* Decode npackets 8-byte packets with a fresh decoder state. LPCNetDecState starts with its LPCNetState
- * (lpcnet_private.h:50-53) so the blob is loaded through that member. */
+ * (lpcnet_private.h:50-53) so the blob is loaded through that member; blob NULL: the compiled-in arrays, as above. */
 int ref_decode_stream(const unsigned char *blob, int len, const unsigned char *packets, int npackets, short *pcm)
 {
     int i;
     LPCNetDecState *st = lpcnet_decoder_create();
-    if (lpcnet_load_model((LPCNetState *)st, blob, len) != 0) { lpcnet_decoder_destroy(st); return -1; }
+    if (blob && lpcnet_load_model((LPCNetState *)st, blob, len) != 0) { lpcnet_decoder_destroy(st); return -1; }
     for (i = 0; i < npackets; i++)
         lpcnet_decode(st, packets + (size_t)i * LPCNET_COMPRESSED_SIZE, pcm + (size_t)i * LPCNET_PACKET_SAMPLES);
     lpcnet_decoder_destroy(st);

@@ -263,6 +263,99 @@ def ref_digest(key, compute, runnable=True):
     return d
 
 
+# ---- models printed in the reference's nnet_data.c / nnet_data.h form (oracle/dump_nnet_data.py) and imported ----
+DUMP_GEN = GEN + "_dump"
+DUMP_REF = os.path.join(ORACLE, "_ref", "dump")
+
+
+@functools.lru_cache(None)
+def dump_dir(model):
+    """oracle/_gen_dump/<model>: nnet_data.c / nnet_data.h of dump_nnet_data.MODELS[model], written on first use."""
+    import dump_nnet_data
+    d = os.path.join(DUMP_GEN, model)
+    if not all(os.path.exists(os.path.join(d, n)) for n in ("nnet_data.c", "nnet_data.h")):
+        dump_nnet_data.write_model(DUMP_GEN, model)
+    return d
+
+
+def _importer():
+    import sys
+    tools = os.path.join(ROOT, "tools")
+    if tools not in sys.path:
+        sys.path.insert(0, tools)
+    import import_nnet_data
+    return import_nnet_data
+
+
+@functools.lru_cache(None)
+def imported(model, kind="int8"):
+    """(blob, arrays, config) of tools/import_nnet_data.py run on the dumped model (kind int8, or float: --float)."""
+    return _importer().import_model(os.path.join(dump_dir(model), "nnet_data.c"), is_float=kind == "float")
+
+
+def have_dump_ref(model, blobs=False):
+    """oracle/Makefile `dumpref` built the reference from this model's nnet_data.c (builds A and B; with blobs: the blobs
+    write_lpcnet_weights wrote)."""
+    files = ("weights_int8.bin", "weights_float.bin") if blobs else ("liblpcnet_ref_A.so", "liblpcnet_ref_B.so")
+    return all(os.path.exists(os.path.join(DUMP_REF, model, f)) for f in files)
+
+
+def dump_ref_blob(model, kind):
+    """The blob write_lpcnet_weights wrote, compiled against the model's nnet_data.c (kind int8: DOT_PROD, float: not)."""
+    return open(os.path.join(DUMP_REF, model, "weights_%s.bin" % kind), "rb").read()
+
+
+@functools.lru_cache(None)
+def _dump_ref_lib(model, build):
+    L = ctypes.CDLL(os.path.join(DUMP_REF, model, "liblpcnet_ref_%s.so" % build))
+    L.ref_synth_batch.argtypes = [ctypes.c_char_p, ctypes.c_int, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p]
+    L.ref_decode_batch.argtypes = [ctypes.c_char_p, ctypes.c_int, c_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_p]
+    return L
+
+
+def dump_ref_synth(model, build, features):
+    """features [n][T][stride] -> pcm [n][T*160] of the reference built from the model's nnet_data.c (build A: int8, B: float)
+    on its compiled-in arrays: no blob is loaded."""
+    f = np.ascontiguousarray(features, dtype=np.float32)
+    n, T, stride = f.shape
+    pcm = np.zeros((n, T * 160), dtype=np.int16)
+    assert _dump_ref_lib(model, build).ref_synth_batch(None, 0, f.ctypes.data, stride, T, n, n, pcm.ctypes.data) == 0
+    return pcm
+
+
+def dump_ref_decode(model, build, packets):
+    """packets [n][P][8] -> pcm [n][P*640], as dump_ref_synth."""
+    p = np.ascontiguousarray(packets, dtype=np.uint8)
+    n, P, _ = p.shape
+    pcm = np.zeros((n, P * 640), dtype=np.int16)
+    assert _dump_ref_lib(model, build).ref_decode_batch(None, 0, p.ctypes.data, P, n, n, pcm.ctypes.data) == 0
+    return pcm
+
+
+def oracle_with_config(model_blob, cfg, features=None, packets=None, nthreads=8):
+    """pcm of the CPU restatement on `model_blob` with the switches cfg = (lpc_gamma, features_delay, end2end): synthesis of
+    features [n][T][stride] or decode of packets [n][P][8]."""
+    L = oracle_lib()
+    m = L.oracle_model_create_ex(model_blob, len(model_blob), rcp_table().ctypes.data, cfg[0], int(cfg[1]), int(cfg[2]),
+                                 codebooks().ctypes.data)
+    assert m, "oracle failed to parse the blob"
+    L.oracle_model_destroy.argtypes = [c_p]
+    try:
+        if features is not None:
+            f = np.ascontiguousarray(features, dtype=np.float32)
+            n, T, stride = f.shape
+            pcm = np.zeros((n, T * 160), dtype=np.int16)
+            L.oracle_synthesize_batch(m, f.ctypes.data, stride, n, T, nthreads, pcm.ctypes.data)
+        else:
+            p = np.ascontiguousarray(packets, dtype=np.uint8)
+            n, P, _ = p.shape
+            pcm = np.zeros((n, P * 640), dtype=np.int16)
+            L.oracle_decode_batch(m, p.ctypes.data, n, P, nthreads, pcm.ctypes.data)
+    finally:
+        L.oracle_model_destroy(m)
+    return pcm
+
+
 def stream_digests(pcm):
     """First 8 bytes of sha256 of every stream's PCM as uint64 [n] (a failing comparison names the stream)."""
     import hashlib

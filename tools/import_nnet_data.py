@@ -79,13 +79,15 @@ def parse_arrays(text, dot_prod=True):
 
 
 def parse_header(text):
-    """LPC_GAMMA, FEATURES_DELAY, END2END from nnet_data.h (dump_lpcnet.py:306-329)."""
+    """LPC_GAMMA, FEATURES_DELAY, END2END from nnet_data.h (dump_lpcnet.py:306-329).  Only live `#define` lines count: a
+    non-end-to-end model's header carries `/* #define END2END */`, and a hand-edited one may keep old values in comments."""
     cfg = {"lpc_gamma": 1.0, "features_delay": 2, "end2end": 0}
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    m = re.search(r"#\s*define\s+LPC_GAMMA\s+([0-9.eE+-]+)f?", text)
+    text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
+    text = re.sub(r"//[^\n]*", "", text)
+    m = re.search(r"^\s*#\s*define\s+LPC_GAMMA\s+([0-9.eE+-]+)f?", text, flags=re.M)
     if m:
         cfg["lpc_gamma"] = float(m.group(1))
-    m = re.search(r"#\s*define\s+FEATURES_DELAY\s+(\d+)", text)
+    m = re.search(r"^\s*#\s*define\s+FEATURES_DELAY\s+(\d+)", text, flags=re.M)
     if m:
         cfg["features_delay"] = int(m.group(1))
     if re.search(r"^\s*#\s*define\s+END2END\b", text, flags=re.M):
